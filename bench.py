@@ -2,6 +2,8 @@
 """bench.py - BASELINE.json's metric on BASELINE.json's configs, one JSON line on stdout.
 
   python bench.py [--gpus N --steps K --warmup W]           our arm (CUDA kernels through the C ABI)
+  python bench.py ... --dump-outputs DIR                     also write what the last timed step of every leg
+                                                             returned as DIR/<name>.npy (float64, fixed samples)
   python bench.py --impl reference [...]                     the reference's CPU operators (oracle/_ref)
 
 Workloads (synthetic TPC-H / SSB-shaped columns, defined once as DuckDB SQL and restated with torch ops in
@@ -21,7 +23,8 @@ bench_data.py, so that both arms see the same rows; row i of rank r is row i + r
            to the stock operators in the same connection.
   cpu_baseline  (N = 1) the reference on the box's usable cores on the first 60 M rows of every workload, with a
            bit-exact comparison of the GPU result on the same rows (`parity`).
-A "step" is one pass of the operator over the whole input.  Every leg lists its K timed steps one by one (`ms_steps`);
+A "step" is one pass of the operator over the whole input.  Every GPU leg times K = --steps steps and lists them one by
+one (`ms_steps`);
 `ms_per_step` / `value` are the K steps as ONE region, the sub-legs' rooflines use the median step.
 `value` = rows/s with inputs resident in HBM;
 `e2e` = the same through the C ABI from pinned HOST buffers (H2D of every input column and D2H of the result
@@ -54,31 +57,58 @@ Q3_INPUT_BYTES_PER_ROW = 19    # i64 + u16 + u8 + i64
 Q3_BYTES_PER_ROW = 51          # SURVEY.md 8d: inputs + one 32 B random state sector per row
 
 
+H100_HBM_GBS = 3350.0          # NVIDIA H100 SXM data sheet (HBM3), not a measured rate
+
+
 def load_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         try:
-            return json.load(open(p)).get("hbm_gbs", 6650.0), "measured (MEASURED_PEAKS.json hbm_gbs)"
+            return json.load(open(p)).get("hbm_gbs", H100_HBM_GBS), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return H100_HBM_GBS, "H100 SXM data sheet (3.35 TB/s HBM3)"
 
 
-def load_traffic():
-    """DRAM bytes per row of the shipped kernels from the committed ncu --set full captures
-    (profiles/r2_traffic.json, written by scripts/ncu_summary.py)."""
-    p = os.path.join(ROOT, "profiles", "r2_traffic.json")
+def gpu_info(device):
+    """name, power limit and max SM clock of the card: an absolute number is only worth something next to them"""
     try:
-        return json.load(open(p))
-    except Exception:
-        return {}
+        out = subprocess.run(["nvidia-smi", "-i", str(device), "--query-gpu=name,power.limit,clocks.max.sm",
+                              "--format=csv,noheader,nounits"], capture_output=True, text=True, timeout=10).stdout
+        f = [x.strip() for x in out.strip().split(",")]
+        return {"name": f[0], "power_limit_w": float(f[1]), "sm_max_mhz": float(f[2])}
+    except Exception as ex:
+        return {"error": f"{type(ex).__name__}: {ex}"}
 
 
-def traffic_of(traffic, key, rows):
-    t = traffic.get(key)
-    if not t:
-        return None, None
-    return int(round(t["dram_bytes_per_row"] * rows)), t.get("source")
+def dump_outputs(outdir, arrays):
+    """--dump-outputs: every array as <outdir>/<name>.npy in float64, at most 64 MB in all.  Integers beyond 2^53 (the
+    128-bit sums) lose their low bits in float64, so such an array is also written exactly as 32-bit limbs:
+    <name>_limb<i>.npy holds bits 32 i .. 32 i + 31 (the top limb signed).  Returns None, or why nothing was written."""
+    out = {}
+    for name, a in arrays.items():
+        a = np.asarray(a)
+        ints = [int(x) for x in a] if a.dtype == object or a.dtype.kind in "iu" else None
+        out[name] = np.asarray(ints if ints is not None else a, dtype=np.float64)
+        if ints and max(abs(x) for x in ints) >= 1 << 53:
+            nlimb = max(2, (max(abs(x) for x in ints).bit_length() + 32) // 32)
+            for i in range(nlimb):
+                out[f"{name}_limb{i}"] = np.array([(x >> (32 * i)) if i == nlimb - 1 else (x >> (32 * i)) & 0xFFFFFFFF
+                                                   for x in ints], dtype=np.float64)
+    total = sum(8 * a.size for a in out.values())
+    if total > 64 << 20:
+        return f"not written: {total} bytes is more than 64 MB"
+    os.makedirs(outdir, exist_ok=True)
+    for name, a in out.items():
+        np.save(os.path.join(outdir, name + ".npy"), a)
+    return None
+
+
+def seeded_positions(n, k, seed):
+    """k fixed positions out of n (all of them when n <= k), in increasing order"""
+    if n <= k:
+        return np.arange(n)
+    return np.sort(np.random.default_rng(seed).choice(n, size=k, replace=False))
 
 
 class ClockSampler:
@@ -279,7 +309,9 @@ def main():
 
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=5)
+    ap.add_argument("--steps", type=int, default=5,
+                    help="timed steps of every GPU leg (>= 1); the CPU legs (--impl reference, cpu_baseline) run on a "
+                         "time budget and take at most 5 / 3 timed runs (their JSON says how many ran)")
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200")
     ap.add_argument("--rows", type=int, default=Q1_ROWS, help="aggregate input rows per GPU")
@@ -295,7 +327,14 @@ def main():
                     help="multi-GPU join plan(s) to measure")
     ap.add_argument("--duckdb-sf", type=float, default=1.0, help="TPC-H scale factor of the e2e_duckdb leg")
     ap.add_argument("--skip", default="", help="comma list of legs to skip: ssb,q3,join,scan,e2e,duckdb,cpu")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the last timed step of each leg returned as DIR/<name>.npy "
+                         "(one GPU only: at N > 1 a caller's result is spread over the ranks)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
+    if args.dump_outputs and int(os.environ.get("WORLD_SIZE", "1")) > 1:
+        ap.error("--dump-outputs needs --gpus 1")
     if args.impl == "reference":
         run_reference_arm(args, emit)
         return
@@ -317,13 +356,13 @@ def main():
     if world > 1:
         os.environ.setdefault("MASTER_ADDR", "127.0.0.1")
         dist.init_process_group("nccl", device_id=dev)
-        # measured on 2 x B200: changing the persisting-L2 carve-out around every probe (b200_l2_pin/unpin) while
-        # NCCL is active costs ~0.4 s per call (and the carve-out is opt-in since round 2 anyway)
+        # changing the persisting-L2 carve-out around every probe (b200_l2_pin/unpin) while NCCL is active costs
+        # ~0.4 s per call (and the carve-out is opt-in)
         os.environ["B200_NO_L2_PIN"] = "1"
     ctx = ops.Context(local_rank, torch.cuda.current_stream().cuda_stream)
     peak, peak_src = load_peaks()
-    traffic = load_traffic()
     K, W = args.steps, max(3, args.warmup)
+    dumps = {}   # --dump-outputs: name -> array
     gen = BD.Gen(torch, dev)
 
     def barrier():
@@ -358,9 +397,8 @@ def main():
         for _ in range(warmup):
             step()
         if True:  # (also with warmup=0: the headline does its own warm-up loop)
-            # one more untimed step AFTER a device-wide synchronise: on this pool the first step that follows a
-            # torch.cuda.synchronize() sometimes stalls once for ~0.1-0.7 s (seen in the scan leg only, per-step times in
-            # `ms_steps` of profiles/r2_bench_n1.json: [101.5, 1.63, 1.58, 1.59, 1.57]); it is not part of any step's work
+            # one more untimed step AFTER a device-wide synchronise: on shared machines the first step that follows a
+            # torch.cuda.synchronize() has been seen to stall once for ~0.1-0.7 s; it is not part of any step's work
             barrier()
             step()
         timed_steps.stalled = None
@@ -375,9 +413,9 @@ def main():
             # the K steps as ONE region (the contract) plus every step on its own (a one-off stall shows up here)
             per_step = [round(ev[i].elapsed_time(ev[i + 1]), 4) for i in range(steps)]
             region = ev[0].elapsed_time(ev[steps])
-            # a single step more than 2 x the median step is a stall of the box, not of the operator (100 ms .. 0.7 s
-            # have been seen on 1.6 .. 10 ms steps): like the driver does for a throttled run, the K-step region is
-            # measured ONCE more and the discarded per-step times are reported next to the kept ones.  Every rank must
+            # a single step more than 2 x the median step is a stall of the machine, not of the operator (100 ms .. 0.7 s
+            # have been seen on 1.6 .. 10 ms steps): the K-step region is measured ONCE more and the discarded
+            # per-step times are reported next to the kept ones.  Every rank must
             # take the same decision (the steps contain collectives).
             stalled = steps >= 3 and max(per_step) > 2.0 * float(np.median(per_step))
             if world > 1:
@@ -391,15 +429,13 @@ def main():
         timed_steps.last = per_step
         return max_over_ranks(region) / steps
 
-    def roofline(bytes_per_row, rows, ms, kernel, traffic_key=None, note=None):
+    def roofline(bytes_per_row, rows, ms, kernel, note=None):
         gbs = bytes_per_row * rows / (ms / 1e3) / 1e9
-        tr, src = traffic_of(traffic, traffic_key, rows) if traffic_key else (None, None)
-        r = {"bound": "hbm", "achieved": gbs, "peak": peak, "unit": "GB/s", "frac": gbs / peak, "traffic": tr,
+        # traffic: measured DRAM bytes (needs a hardware-counter profiler; None = not measured)
+        r = {"bound": "hbm", "achieved": gbs, "peak": peak, "unit": "GB/s", "frac": gbs / peak, "traffic": None,
              "kernel": kernel, "ms": ms, "peak_source": peak_src, "bytes_per_row": bytes_per_row,
              "ms_stat": "headline: mean of the K sink calls; other legs: MEDIAN of the K timed steps / sink calls (every "
-                        "step is in ms_steps; the shared boxes of this pool show one-off stalls of 8-700 ms in single steps)"}
-        if src:
-            r["traffic_source"] = src
+                        "step is in ms_steps; shared machines show one-off stalls of 8-700 ms in single steps)"}
         if note:
             r["note"] = note
         return r
@@ -489,7 +525,12 @@ def main():
         return f"bit-exact on {m} rows ({len(got)} groups: 4 hugeint sums + count, 3 avgs within 1e-9)"
 
     checks["q1"] = check_q1
-    tr, trsrc = traffic_of(traffic, "agg_fastreg", n)
+    if args.dump_outputs:
+        # SELECT rf, ls, sum(qty), sum(price), sum(disc_price), sum(charge), avg(qty), avg(price), avg(disc), count(*)
+        order = np.lexsort((res[1][0].astype(np.int64), res[0][0].astype(np.int64)))
+        for i, nme in enumerate(("rf", "ls", "sum_qty", "sum_price", "sum_disc_price", "sum_charge", "avg_qty",
+                                 "avg_price", "avg_disc", "count")):
+            dumps["agg_q1_" + nme] = res[i][0][order]
     line = {
         "metric": "agg_input_rows_per_s", "value": agg_value, "unit": "rows/s", "n_gpus": world, "steps": K,
         "warmup": W, "ms_per_step": agg_ms, "ms_steps": agg_steps_ms, "ms_steps_discarded": agg_stalled, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
@@ -501,9 +542,8 @@ def main():
                    "combine": "none (N = 1)" if world == 1 else "all-gather of packed partial states + one merge kernel, "
                                                                 "inside every timed step"},
         "roofline": roofline(AGG_BYTES_PER_ROW, n, sink_ms,
-                             "agg_fastreg_kernel<5,4,224,1> (b200_agg_sink, incl. the 256 K-row adaptation probe)",
-                             "agg_fastreg"),
-        "gpu_launches": int(launches), "clocks": clocks,
+                             "agg_fastreg_kernel<5,4,224,1> (b200_agg_sink, incl. the 256 K-row adaptation probe)"),
+        "gpu_launches": int(launches), "clocks": clocks, "gpu": gpu_info(local_rank),
     }
 
     # ----------------------------------------------------------------- e2e aggregate (host buffers)
@@ -540,16 +580,15 @@ def main():
         s0 = ctx.stats()
         barrier()
         w0 = time.perf_counter()
-        ksteps = max(1, min(K, 3))
-        for _ in range(ksteps):
+        for _ in range(K):
             r2 = e2e_step()
         barrier()
-        e2e_s = max_over_ranks(time.perf_counter() - w0) / ksteps
+        e2e_s = max_over_ranks(time.perf_counter() - w0) / K
         s1 = ctx.stats()
         assert int(r2[9][0].sum()) == n * world
-        line["e2e"] = {"value": world * n / e2e_s, "unit": "rows/s",
-                       "h2d_bytes_per_step": int((s1["h2d_bytes"] - s0["h2d_bytes"]) // ksteps),
-                       "d2h_bytes_per_step": int((s1["d2h_bytes"] - s0["d2h_bytes"]) // ksteps),
+        line["e2e"] = {"value": world * n / e2e_s, "unit": "rows/s", "steps": K,
+                       "h2d_bytes_per_step": int((s1["h2d_bytes"] - s0["h2d_bytes"]) // K),
+                       "d2h_bytes_per_step": int((s1["d2h_bytes"] - s0["d2h_bytes"]) // K),
                        "ms_per_step": e2e_s * 1e3, "h2d_gbs_per_gpu": AGG_BYTES_PER_ROW * n / e2e_s / 1e9,
                        "note": "pinned host columns -> b200_batch_upload (64 Mi-row morsels) -> sink -> "
                                + ("cross-rank combine -> " if world > 1 else "") + "finalize -> D2H of the result"}
@@ -587,6 +626,10 @@ def main():
         steps_ms = list(timed_steps.last)
         stalled_ms = timed_steps.stalled
         sink = float(np.median([a.elapsed_time(b) for a, b in ev[-K:]]))   # median: a one-off stall is not the kernel
+        if args.dump_outputs:
+            order = np.lexsort((step.res[1][0].astype(np.int64), step.res[0][0].astype(np.int64)))
+            for i, nme in enumerate(("year", "nation", "sum_profit")):
+                dumps["agg_ssb_" + nme] = step.res[i][0][order]
         got = groups_of(step.res, 2)
         assert len(got) == 35, len(got)
         assert sum(int(v[0]) for v in got.values()) == sum_over_ranks(int(d["profit"].sum().item())), "sum(profit) mismatch"
@@ -606,8 +649,7 @@ def main():
             "config": {"workload": "SSB Q4.1-shaped aggregate (BASELINE configs[4]'s group-by): GROUP BY d_year, c_nation "
                                    "SUM(lo_revenue - lo_supplycost); every row of an SF100-sized shard (stress)",
                        "rows_per_gpu": ns, "row_bytes": SSB_BYTES_PER_ROW, "groups": 35},
-            "roofline": roofline(SSB_BYTES_PER_ROW, ns, sink, "agg_priv_kernel<1,0> (thread-private shared-memory accumulators)",
-                                 "agg_priv1")}
+            "roofline": roofline(SSB_BYTES_PER_ROW, ns, sink, "agg_priv_kernel<1,0> (thread-private shared-memory accumulators)")}
         checks["_keep_ssb"] = (cols, batch)
 
     if "ssb" not in skip:
@@ -655,6 +697,12 @@ def main():
         sink = float(np.median([a.elapsed_time(b) for a, b in ev[-K:]]))   # median: a one-off stall is not the kernel
         tot_groups = sum_over_ranks(step.groups)
         res = step.out.download_all()
+        if args.dump_outputs:
+            # groups in key order, a fixed sample of 200 K of them
+            order = np.lexsort((res[2][0].astype(np.int64), res[1][0].astype(np.int64), res[0][0].astype(np.int64)))
+            pick = order[seeded_positions(len(order), 200_000, 3)]
+            for i, nme in enumerate(("okey", "odate", "prio", "sum_revenue")):
+                dumps["agg_q3_" + nme] = res[i][0][pick]
         tot_sum = sum_over_ranks(sum(int(x) for x in res[3][0]))
         assert tot_sum == sum_over_ranks(int(d["revenue"].sum().item())), "sum(revenue) mismatch"
         if world == 1:
@@ -683,9 +731,10 @@ def main():
                        "groups": groups,
                        "plan": "local" if world == 1 else "rows shuffled by key radix (all-to-all), local aggregate, no merge"},
             "roofline": roofline(Q3_BYTES_PER_ROW, nq, sink, "agg_hc_direct_kernel<2,1> (L2-first structure-of-arrays table; "
-                                 "sink incl. the adaptation probe, chunking and table growth)", "agg_hc",
+                                 "sink incl. the adaptation probe, chunking and table growth)",
                                  note="SURVEY 8d's 51 B/row: 19 B of inputs + one 32 B random state sector per row; the table "
-                                      "(1 M groups = 48 MB) stays in L2, so DRAM traffic is the 19 B/row of inputs")}
+                                      "(1 M groups = 48 MB) is about the size of the H100's 50 MB L2, so part of it is "
+                                      "served from HBM while the input streams past; how much is not measured")}
         checks["_keep_q3"] = (cols, batch)
 
     if "q3" not in skip:
@@ -705,6 +754,28 @@ def main():
         pk, pprice, pdisc = probe["partkey"], probe["price"], probe["disc"]
         bbatch = wrap([bk, bp], [capi.INT64, capi.UINT8], nb)
         pbatch = wrap([pk, pprice, pdisc], [capi.INT64] * 3, npb)
+
+        def dump_join(o, name):
+            """the joined (price, disc, promo) rows come out in no fixed order: keep the rows whose content hashes
+            to 0 mod 1024 (a sample that does not depend on the order) and sort them"""
+            from duckdb_b200.distributed import _DevArray
+
+            c = o.nrows
+            price, disc, promo = (torch.as_tensor(_DevArray(o.column_info(i).data, c, t), device=dev)
+                                  for i, t in ((0, "<i8"), (1, "<i8"), (2, "|u1")))
+            parts = []
+            for lo in range(0, c, 1 << 26):   # in chunks: the inputs of every leg are still resident
+                p_, d_, m_ = price[lo:lo + (1 << 26)], disc[lo:lo + (1 << 26)], promo[lo:lo + (1 << 26)].to(torch.int64)
+                h = p_ * 1000003 + d_ * 131 + m_
+                h = (h ^ (h >> 29)) * 0x5851F42D4C957F2D
+                keep = ((h ^ (h >> 32)) & 1023) == 0
+                parts.append(torch.stack([p_[keep], d_[keep], m_[keep]]).cpu().numpy())
+            rows = np.concatenate(parts, axis=1) if parts else np.zeros((3, 0), dtype=np.int64)
+            order = np.lexsort(rows[::-1])
+            for i, nme in enumerate(("price", "disc", "promo")):
+                dumps[f"{name}_{nme}_sample"] = rows[i][order]
+
+        main_plan = "local" if world == 1 else ("broadcast" if args.join_plan == "both" else args.join_plan)
 
         def run_plan(plan):
             j = ops.HashJoin(ctx, capi.JOIN_INNER, [capi.INT64], [capi.UINT8])
@@ -743,6 +814,9 @@ def main():
 
             def probe_step():
                 probe_step.sum = 0
+                if probe_step.last is not None:
+                    probe_step.last.free()
+                    probe_step.last = None
                 if pipe is not None:
                     def consume(o, c):
                         if probe_step.check:
@@ -761,12 +835,22 @@ def main():
                 probe_step.cnt = c
                 if probe_step.check:
                     probe_step.sum = checksum(o)
-                o.free()
+                if probe_step.keep:
+                    probe_step.last = o
+                else:
+                    o.free()
 
             probe_step.check = False
+            probe_step.last = None
+            probe_step.keep = bool(args.dump_outputs) and pipe is None and rank == 0
             ms = timed_steps(probe_step)
             steps_ms = list(timed_steps.last)
             stalled_ms = timed_steps.stalled
+            if probe_step.last is not None:
+                dump_join(probe_step.last, "join_probe_" + plan if plan != main_plan else "join_probe")
+                probe_step.last.free()
+                probe_step.last = None
+            probe_step.keep = False
             probe_step.check = True
             probe_step()   # one more, untimed, with the checksum of the joined column
             assert sum_over_ranks(probe_step.cnt) == npb * world, (probe_step.cnt, npb)
@@ -781,7 +865,7 @@ def main():
         results = {}
         for p in plans:
             results[p] = run_plan(p)
-        main_plan = plans[0]
+        assert main_plan == plans[0]
         r = results[main_plan]
         dense_note = ("achieved uses SURVEY 8d's 73 B/row; with the dense (perfect-hash) table the 32 B random sector is a "
                       "4 B L2-resident entry, i.e. 45 B/row actually move")
@@ -801,7 +885,7 @@ def main():
                        "hash_table_rows_per_gpu": nb_total if main_plan == "broadcast" else nb, "probe_rows_per_gpu": npb,
                        "row_bytes": JOIN_BYTES_PER_ROW, "l2": "probe inputs (14.4 GB) larger than L2"},
             "build_ms": r["build_ms"], "build_rows_per_s": world * nb / (r["build_ms"] / 1e3),
-            "roofline": roofline(JOIN_BYTES_PER_ROW, npb, float(np.median(r["ms_steps"])), "join_probe_lean2_kernel<2,8,dense>", "join_dense",
+            "roofline": roofline(JOIN_BYTES_PER_ROW, npb, float(np.median(r["ms_steps"])), "join_probe_lean2_kernel<2,8,dense>",
                                  note=dense_note)}
         for p in plans[1:]:
             q = results[p]
@@ -811,7 +895,7 @@ def main():
                 "n_gpus": world, "plan": plan_text[p], "build_ms": q["build_ms"],
                 "nvlink_bytes_per_step_per_gpu": int(npb * 24 * (world - 1) / world),
                 "roofline": roofline(JOIN_BYTES_PER_ROW, npb, q["ms"], "part_count + part_move_staged + all-to-all + "
-                                                                         "join_probe_tile_kernel", None)}
+                                                                         "join_probe_tile_kernel")}
 
         def check(m, nbs, ref_rows):
             """first m probe rows against a build side of nbs keys (the reference's bounded sample)"""
@@ -863,14 +947,16 @@ def main():
             s0 = ctx.stats()
             barrier()
             w0 = time.perf_counter()
-            tot = join_e2e()
+            for _ in range(K):
+                tot = join_e2e()
             barrier()
-            dt = time.perf_counter() - w0
+            dt = (time.perf_counter() - w0) / K
             s1 = ctx.stats()
             assert tot == npb
-            line["join_probe"]["e2e"] = {"value": npb / dt, "unit": "rows/s",
-                                         "h2d_bytes_per_step": int(s1["h2d_bytes"] - s0["h2d_bytes"]),
-                                         "d2h_bytes_per_step": int(s1["d2h_bytes"] - s0["d2h_bytes"]), "ms_per_step": dt * 1e3}
+            line["join_probe"]["e2e"] = {"value": npb / dt, "unit": "rows/s", "steps": K,
+                                         "h2d_bytes_per_step": int((s1["h2d_bytes"] - s0["h2d_bytes"]) // K),
+                                         "d2h_bytes_per_step": int((s1["d2h_bytes"] - s0["d2h_bytes"]) // K),
+                                         "ms_per_step": dt * 1e3}
             del hk, hp, hd, hnp
         for q in results.values():
             q["join"].close()
@@ -890,6 +976,9 @@ def main():
         fp = ops.FilterProject(ctx, e, root, [e.col(1, capi.INT64)])
 
         def step():
+            if step.o is not None:
+                step.o.free()
+                step.o = None
             o, c, _, _ = fp.execute(sb)
             step.c = c
             step.sum = None
@@ -898,7 +987,8 @@ def main():
             else:
                 o.free()
 
-        step.keep = False
+        step.o = None
+        step.keep = bool(args.dump_outputs)
         if os.environ.get("BENCH_SCAN_DIAG"):
             def log(msg):
                 sys.stderr.write(msg + "\n")
@@ -922,6 +1012,17 @@ def main():
         scan_steps = list(timed_steps.last)
         scan_stalled = timed_steps.stalled
         c = step.c
+        if step.o is not None:
+            # the surviving l_quantity values keep the input's row order: a fixed sample of 1 M positions
+            from duckdb_b200.distributed import _DevArray
+
+            qty = torch.as_tensor(_DevArray(step.o.column_info(0).data, c, "<i8"), device=dev)
+            pos = torch.as_tensor(seeded_positions(c, 1 << 20, 5), device=dev)
+            dumps["scan_qty_sample"] = qty[pos].cpu().numpy()
+            dumps["scan_count"] = np.array([c])
+            step.o.free()
+            step.o = None
+        step.keep = False
         assert c == int((shipdate < 8766).sum().item()), "scan count mismatch"
         scan_bytes = ns * 12 + c * 8
         line["scan"] = {"metric": "scan_filter_rows_per_s", "value": world * ns / (scan_ms / 1e3), "unit": "rows/s",
@@ -930,7 +1031,7 @@ def main():
                                    "rows_per_gpu": ns, "parallelism": f"row-range shard{world}, no collective"},
                         "roofline": roofline(scan_bytes / ns, ns, float(np.median(scan_steps)),
                                              "filter_mask_tile_kernel<32> + tile_scan + compact_tile_kernel "
-                                             "(B200_FILTER_FUSED=1: filter_fused_tile_kernel)", None)}
+                                             "(B200_FILTER_FUSED=1: filter_fused_tile_kernel)")}
         # the same predicate with l_shipdate as a DICTIONARY vector (2526 distinct dates + one uint32 index per row, what
         # DuckDB hands over for dictionary-compressed segments): generic expression interpreter (csrc/filter.cu)
         dvals = torch.arange(8036, 8036 + 2526, device=dev, dtype=torch.int32)
@@ -943,17 +1044,13 @@ def main():
             dstep.c = cc
             o.free()
 
-        dict_ms = timed_steps(dstep, warmup=2, steps=3)
+        dict_ms = timed_steps(dstep, warmup=2)
         assert dstep.c == c, "dictionary-vector scan count mismatch"
         line["scan"]["dictionary_vector"] = {"value": world * ns / (dict_ms / 1e3), "unit": "rows/s", "ms_per_step": dict_ms,
                                              "kernel": "filter_mask_kernel + compact_kernel (generic interpreter: per-row "
                                                        "vector-type dispatch, dictionary gather)",
                                              "achieved_gbs": (ns * 12 + c * 8) / (dict_ms / 1e3) / 1e9}
         del dbatch, dsel
-        tm, tc_ = traffic.get("filter_mask"), traffic.get("filter_compact")
-        if tm and tc_:
-            line["scan"]["roofline"]["traffic"] = int(round((tm["dram_bytes_per_row"] + tc_["dram_bytes_per_row"]) * ns))
-            line["scan"]["roofline"]["traffic_source"] = "profiles/r2_filter_mask_ncu.txt + profiles/r2_filter_compact_ncu.txt"
 
         def check(m, ref_rows):
             o, cc, _, _ = fp.execute(wrap([shipdate, quantity], [capi.INT32, capi.INT64], m))
@@ -1012,7 +1109,7 @@ def main():
             plan = "\n".join(str(r[-1]) for r in con.fetchall("EXPLAIN " + sql))
             rows = con.fetchall(sql)
             ts = []
-            for _ in range(3):
+            for _ in range(K):
                 t0 = time.perf_counter()
                 con.fetchall(sql)
                 ts.append(time.perf_counter() - t0)
@@ -1063,6 +1160,10 @@ def main():
             traceback.print_exc()
             line["cpu_baseline"] = {"value": None, "unit": "rows/s", "cores": 0, "kind": "reference",
                                     "sample": f"failed: {type(ex).__name__}: {ex}"}
+    if args.dump_outputs and rank == 0:
+        err = dump_outputs(args.dump_outputs, dumps)
+        if err:
+            line["dump_outputs"] = {"error": err}
     if rank == 0:
         emit(line)
     if world > 1:

@@ -1,6 +1,6 @@
-"""duckdb_b200: B200-native kernels for DuckDB's hash-join, hash-aggregate and filter/projection operators.
+"""duckdb_b200: H100-native kernels for DuckDB's hash-join, hash-aggregate and filter/projection operators.
 
-The product is duckdb_b200/_lib/libduckdb_b200.so (CUDA sm_100a + C ABI, include/duckdb_b200.h);
+The product is duckdb_b200/_lib/libduckdb_b200.so (CUDA sm_90a + C ABI, include/duckdb_b200.h);
 this package is the thin host-side mirror of the reference's operator interface over that ABI.
 """
 from . import capi  # noqa: F401

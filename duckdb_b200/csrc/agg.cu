@@ -4,7 +4,7 @@
 // CombineStates / FinalizeStates (src/common/row_operations/row_aggregate.cpp:52-64,120-150),
 // sum / avg / count / min / max state arithmetic (extension/core_functions/aggregate/distributive/sum.cpp,
 // include/core_functions/aggregate/sum_helpers.hpp:107-215, algebraic/avg.cpp:84-140).
-// Design (B200-first, not the reference's pointer-table + row store): ONE open-addressing table whose slot
+// Design (GPU-first, not the reference's pointer-table + row store): ONE open-addressing table whose slot
 // row holds [tag | packed key | shared aggregate states], so a row update touches one or two 32-byte sectors.
 // Three sink paths, chosen adaptively per aggregate (the analogue of RadixPartitionedHashTable::DecideAdaptation,
 // radix_partitioned_hashtable.cpp:533-571):

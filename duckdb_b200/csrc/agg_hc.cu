@@ -1,9 +1,8 @@
 // K6 sink path HC: high-cardinality groups (TPC-H Q3: millions of groups) in an L2-FIRST structure-of-arrays table.
 //
-// Measured on B200 (scripts/ubench/atomics.cu, profiles/r2_ubench_atomics.txt): what a random table access costs is
-// the NUMBER of L2 transactions per row and whether the touched footprint stays inside the 126 MB L2 - not sector
-// locality.  L2-resident: one 16-byte load + one RED = 74 G rows/s, + a second RED = 52 G rows/s; the same ops on a
-// 1 GB table = 15 / 14 G rows/s.  The generic table of agg.cu (one 64-128 byte row per group holding tag, key, hash,
+// What a random table access costs is the NUMBER of L2 transactions per row and whether the touched footprint stays
+// inside L2 (50 MB on an H100) - not sector locality; scripts/ubench/atomics.cu measures both against the table size
+// (not yet run on H100).  The generic table of agg.cu (one 64-128 byte row per group holding tag, key, hash,
 // rows, cnt and 128-bit sums updated with value-returning atomics) costs ~6 transactions per row and outgrows L2 at
 // 1 M groups.  This path therefore keeps, per group, only what the row path touches, each in its own dense array:
 //   keys[cap][KW]  the packed group key (1 or 2 words); bits 6/7 of its NULL-flag byte are OCCUPIED / LOCKED, so the
@@ -12,7 +11,8 @@
 //   B[i][cap]      per summed input: sum of the values' HIGH 32 bits  (RED only when that half is non-zero: DECIMAL /
 //                  BIGINT measures below 2^32 never touch it)          sum = A + (B << 32) in 128 bits
 //   rows[cap]      only when an aggregate needs a count (COUNT / COUNT(*) / AVG); cnt[i][cap] only for nullable inputs
-// TPC-H Q3's group-by (keys i64 + u16 + u8, one SUM): 16 B load + 1 RED per row; 1 M groups = 48 MB, L2-resident.
+// TPC-H Q3's group-by (keys i64 + u16 + u8, one SUM): 16 B load + 1 RED per row; 1 M groups = 48 MB, about the size of
+// an H100's 50 MB L2, so with the input streaming past it cannot all stay resident (how much does is not measured).
 // The table is an accumulation front end: b200_agg_finalize / export / combine first merge it into the generic table
 // (agg_hc_flush_kernel), so everything downstream of the sink is unchanged.  Rows that find the table at its fill
 // limit are DEFERRED (their row ids are appended to a list, one atomic per warp); the host doubles the table (rehash)
@@ -138,7 +138,7 @@ __device__ __forceinline__ uint64_t hc_find_or_create(const HcView &H, const uin
 				return slot; // the key is the whole block: nothing else to wait for (state arrays start zeroed)
 			}
 			// Hit path (every row after the first of its group): the block's words came from ONE aligned 16-byte load
-			// of a published slot - no fence (a membar per row was the hottest stall in ncu, ERRBAR).  Only a slot seen
+			// of a published slot - no fence (a membar per row would be the hottest stall).  Only a slot seen
 			// while its inserter still holds the lock waits, fences and re-reads.
 			bool eq = !(last & H.lock_bit);
 #pragma unroll
@@ -218,8 +218,7 @@ __device__ __forceinline__ void hc_defer_rows(uint32_t *deferred, unsigned long 
 // One probe step of row state (slot, w[]): -1 = keep probing (slot advanced, next key block loaded), else the slot or
 // SLOT_DEFER.  The body of hc_find_or_create's loop, split out so that a thread can advance ALL its rows one step per
 // round: the rows' dependent L2 loads overlap, and a warp's trip count is the longest probe sequence of any of its
-// rows instead of the sum over the rows of the per-row maxima (ncu, first version: 13.6 of 32 lanes active on
-// average, 1300 warp instructions per row).
+// rows instead of the sum over the rows of the per-row maxima (per-lane probe loops leave most lanes idle).
 #define HC_PENDING 0xfffffffffffffffeULL
 template <int KW>
 __device__ __forceinline__ uint64_t hc_probe_step(const HcView &H, const uint64_t kw[KEY_WORDS_MAX], uint64_t &slot,
@@ -354,8 +353,8 @@ __global__ void __launch_bounds__(HC_THREADS + 32, 2)
 // Integer keys without NULLs (<= 4 key columns) and <= 4 INT64 / UINT64 inputs without NULLs: the TPC-H / SSB shape.
 // Same table protocol as agg_hc_kernel, but the hot loop holds nothing but the hit path: keys are packed from four
 // predicated descriptor slots, the slot hash is one multiply-xorshift-multiply, inserts / locked slots / full tables go
-// through ONE out-of-line call (hc_slow_path), the deferral list is built from a bit mask.  ncu on the generic kernel:
-// 945 warp instructions per 32 rows, issue-bound; this one is built to stay below ~150.
+// through ONE out-of-line call (hc_slow_path), the deferral list is built from a bit mask.  The generic kernel is issue-bound; this
+// one keeps the instructions per row several times lower.
 struct HcSimple {
 	TileCols tc;
 	int stages;
@@ -518,7 +517,7 @@ __global__ void __launch_bounds__(HC_THREADS + 32, 2)
 // The table accesses are random L2 round trips; what hides them is the NUMBER of independent rows in flight, not a
 // staged input pipeline.  This variant has no shared memory and no tile loop: every thread takes one row at a time
 // (grid-stride, coalesced direct loads of the narrow input columns), 32-48 resident warps per SM.  It is the shape of
-// the atomics micro-benchmark that reaches 64-74 G rows/s on an L2-resident table.
+// the atomics micro-benchmark (scripts/ubench/atomics.cu).
 struct HcDirect {
 	int nkeys, ninputs;
 	const unsigned char *key_ptr[4];
@@ -1070,10 +1069,10 @@ int b200_agg_hc_sink(b200_ctx *ctx, AggHc *hc, const AggLayout &L, const KeyCols
 	if (n == 0) {
 		return B200_OK;
 	}
-	// keep the hot arrays of an L2-sized table in the persisting part of L2 while rows stream past
-	// (opt-in: measured on B200 it does nothing for a 48 MB table - 30.4 vs 30.9 G rows/s, the streaming loads already
-	// keep it resident - and it halves the throughput of tables that outgrow the window: B200_HC_L2_PIN=1)
-	if (getenv("B200_HC_L2_PIN") && hc->pinned_mem != hc->mem && hc->hot_bytes <= ((size_t)96 << 20) &&
+	// keep the hot arrays of a table that fits three quarters of L2 in the persisting part of L2 while rows stream past
+	// (opt-in, B200_HC_L2_PIN=1: pinning a table that outgrows the window slows the sink down; the effect on H100 is
+	// not measured)
+	if (getenv("B200_HC_L2_PIN") && hc->pinned_mem != hc->mem && hc->hot_bytes <= ctx->l2_size / 4 * 3 &&
 	    !getenv("B200_NO_L2_PIN")) {
 		b200_l2_pin(ctx, hc->mem, hc->hot_bytes);
 		hc->pinned_mem = hc->mem;

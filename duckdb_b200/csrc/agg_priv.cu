@@ -1,8 +1,7 @@
 // K6 sink path PRIV: thread-private accumulators in shared memory for ~9..64 groups (SSB Q4.1: 35 groups).
 //
-// Why not shared-memory atomics (MID): measured on B200 an ATOMS costs ~2 cycles per LANE (64 cycles per warp
-// instruction), so a row with S sums pays 2 x (1 + 4 S) cycles per SM - MID tops out near 10 G rows/s for the
-// 5-sum shape - while plain LDS / STS move 128 B per cycle.  So, like the register path (FASTREG) but with the
+// Why not shared-memory atomics (MID): a shared-memory atomic is serviced per LANE, so a row with S sums pays for
+// 1 + 4 S lane-serialised updates per SM, while plain LDS / STS move 128 B per cycle.  So, like the register path (FASTREG) but with the
 // states in shared memory: every consumer thread owns a private copy of the state of every slot, laid out
 // [slot][sum][thread] (a warp's accesses hit 32 consecutive 8-byte words: conflict free).  A row costs one lookup in
 // a small CTA-wide directory (packed key -> slot) and, per sum, LDS.64 + IADD.64 + STS.64.  No atomics, no shuffles
@@ -67,8 +66,8 @@ __device__ __forceinline__ int priv_lookup(PrivShared &S, unsigned long long *sl
 }
 
 // DIRECT addressing, one key column of width sizeof(T), PRIV_RB rows: slot += lut[value - min] * stride.  The width
-// dispatch sits OUTSIDE the row loop (ncu on the per-row generic decode: 193 instructions per row for 2 keys + 1 sum,
-// two thirds of them key decoding).
+// dispatch sits OUTSIDE the row loop (decoding the key per row with run-time widths costs more instructions than the
+// rest of the row's work).
 template <class T>
 __device__ __forceinline__ void direct_codes(const unsigned char *col, const uint8_t *lut, uint64_t kmin64, uint32_t range,
                                              uint32_t stride, const uint32_t (&row)[PRIV_RB], int (&sl)[PRIV_RB],
@@ -314,7 +313,7 @@ __global__ void __launch_bounds__(512 + 32, 1)
 
 // ------------------------------------------------------------------ WPRIV: warp-private accumulators
 // PRIV gives every THREAD its own copy of every slot: 35 groups x 5 sums need 1.5 KB per thread, so only 96 threads
-// fit an SM and the kernel crawls (20 G rows/s).  WPRIV keeps one copy per WARP ([warp][slot][sum]: 16 warps x 36
+// fit an SM and the kernel crawls.  WPRIV keeps one copy per WARP ([warp][slot][sum]: 16 warps x 36
 // slots x 5 sums = 23 KB) and lets the lanes of a warp that hit the same slot take turns: ONE match.any tells every
 // lane which lanes share its slot, lane `rank r` of each such set updates the state in round r with plain
 // LDS / IADD / STS - in a round every active lane works on a different slot, so there is nothing to lose and nothing
@@ -637,8 +636,8 @@ int b200_agg_priv_launch(b200_ctx *ctx, TileArgs &A, const AggLayout &L, const K
 	if (slots < 8) {
 		slots = 8;
 	}
-	// thread-private copies win when >= 256 threads' worth of them fit (measured, SSB shape, 36 slots x 1 sum: 88.7 G
-	// rows/s against 68 with warp-private copies); otherwise the warp-private variant (35 groups x 5 sums: 48 against 20)
+	// thread-private copies when >= 256 threads' worth of them fit (no bank conflicts, no rounds); otherwise the
+	// warp-private variant
 	bool thread_private_fits = false;
 	if (PD.nslots) {
 		uint32_t tr0 = 0;

@@ -9,7 +9,7 @@
 //   table with one atomic per (CTA, group, state).
 // MID  (<= ~1-2 K groups per CTA; SSB Q4.1: 35 groups)
 //   A per-CTA open-addressing table in shared memory; 128-bit sums are four 32-bit words updated with native
-//   32-bit ATOMS and explicit carry propagation (64-bit shared atomics are CAS loops on sm_100).
+//   32-bit ATOMS and explicit carry propagation (64-bit shared atomics are CAS loops).
 // Rows that do not fit the per-CTA structure take the global path inline (agg_find_or_create + global atomics)
 // and are counted in counters[1] so the host can switch path (b200_agg_sink's adaptation).
 //
@@ -1055,7 +1055,7 @@ int b200_agg_tile_sink(b200_ctx *ctx, int mode, int slots_hint, const AggLayout 
 			// two CTAs per SM: deeper ring of smaller tiles (3 x 512 rows) when it fits, else 2 x 1024
 			uint32_t rows = tile_env && atoi(tile_env) >= 128 ? (uint32_t)atoi(tile_env) / 128 * 128 : 1024;
 			tile_cols_finish(&A.tc, rows);
-			A.stages = 3; // measured on B200: 2 x 1024-row stages beat 3 x 512 (per-tile issue cost), see profiles/
+			A.stages = 3; // falls back to 2 stages when 3 do not fit the budget below
 			if ((size_t)A.stages * A.tc.stage_bytes > 108 * 1024) {
 				A.stages = 2;
 			}

@@ -1,4 +1,4 @@
-// Shared device/host definitions for the B200 operator kernels.
+// Shared device/host definitions for the operator kernels (H100, sm_90a).
 // Layout notes live in DESIGN.md ("Data layout in HBM").
 #pragma once
 #include <cuda_runtime.h>
@@ -7,7 +7,7 @@
 #include <vector>
 #include "../../include/duckdb_b200.h"
 
-#define B200_SM_COUNT 148
+#define B200_SM_COUNT 132 // H100 SXM; only a fallback, the context reads the device attribute
 
 // ----------------------------------------------------------------- errors
 void b200_set_error(const char *fmt, ...);
@@ -53,6 +53,7 @@ struct b200_ctx {
 	uint64_t *dev_scratch; // 64 words
 	size_t l2_persist_max;  // bytes of L2 that may be set aside for persisting accesses (0 = unsupported)
 	size_t l2_window_max;   // largest access-policy window
+	size_t l2_size;         // bytes of L2 (cudaDevAttrL2CacheSize; 50 MB on an H100 SXM)
 };
 
 // Pin [ptr, ptr+bytes) in L2 for the kernels launched next on the context's stream (hash tables that are re-used

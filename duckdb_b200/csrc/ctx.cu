@@ -38,7 +38,7 @@ const char *b200_last_error(void) {
 }
 
 const char *b200_version(void) {
-	return "duckdb_b200 0.1 (sm_100a)";
+	return "duckdb_b200 0.1 (sm_90a)";
 }
 
 int b200_device_count(void) {
@@ -96,8 +96,7 @@ int b200_ctx_create(int device, void *stream, b200_ctx **out) {
 		uint64_t thresh = UINT64_MAX;
 		cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &thresh);
 	}
-	// experiment knob: B200_L2_FETCH=32|64|128 sets cudaLimitMaxL2FetchGranularity (measured on B200: 32 B makes
-	// the join probe SLOWER than the default, see profiles/README.md, so the default is left alone)
+	// experiment knob: B200_L2_FETCH=32|64|128 sets cudaLimitMaxL2FetchGranularity (the default is left alone)
 	{
 		const char *env = getenv("B200_L2_FETCH");
 		if (env && atoi(env) > 0) {
@@ -109,6 +108,10 @@ int b200_ctx_create(int device, void *stream, b200_ctx **out) {
 	{
 		int v = 0;
 		ctx->l2_persist_max = ctx->l2_window_max = 0;
+		ctx->l2_size = (size_t)50 << 20;
+		if (cudaDeviceGetAttribute(&v, cudaDevAttrL2CacheSize, device) == cudaSuccess && v > 0) {
+			ctx->l2_size = (size_t)v;
+		}
 		if (cudaDeviceGetAttribute(&v, cudaDevAttrMaxPersistingL2CacheSize, device) == cudaSuccess && v > 0) {
 			ctx->l2_persist_max = (size_t)v;
 		}
@@ -116,10 +119,9 @@ int b200_ctx_create(int device, void *stream, b200_ctx **out) {
 			ctx->l2_window_max = (size_t)v;
 		}
 		cudaGetLastError();
-		// Opt-in (B200_L2_PIN=1).  With the lean probe kernels (evict-first streaming loads) pinning the table buys
-		// nothing any more (Q14 probe 9.60 ms pinned vs 9.66 ms not), while the carve-out survives the operator in ways
-		// the runtime does not undo reliably: the filter scan that followed a pinned probe in the same process ran at
-		// 4 ms .. 95 ms instead of 2.0 ms (profiles/README.md).
+		// Opt-in (B200_L2_PIN=1).  The lean probe kernels read their input with evict-first streaming loads, and the
+		// carve-out survives the operator in ways the runtime does not undo reliably, so it can slow down the
+		// operators that run after a pinned probe in the same process.
 		if (!getenv("B200_L2_PIN") || getenv("B200_NO_L2_PIN")) {
 			ctx->l2_persist_max = 0;
 		}
@@ -281,8 +283,8 @@ void b200_l2_unpin(b200_ctx *ctx) {
 	memset(&attr, 0, sizeof(attr));
 	attr.accessPolicyWindow.num_bytes = 0;
 	cudaStreamSetAttribute(ctx->stream, cudaStreamAttributeAccessPolicyWindow, &attr);
-	// give the persisting lines AND the carve-out back: a standing carve-out / stale persisting lines slowed the next
-	// operator down (measured: filter scan 4.2 -> 5.6 -> 32 ms after a pinned probe), see profiles/README.md
+	// give the persisting lines AND the carve-out back: a standing carve-out / stale persisting lines slow the next
+	// operator down
 	if (!getenv("B200_L2_KEEP")) {
 		cudaCtxResetPersistingL2Cache();
 		cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, 0);

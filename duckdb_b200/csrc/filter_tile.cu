@@ -80,8 +80,8 @@ __device__ __forceinline__ void eval_term_rows(const unsigned char *col, int tid
 }
 
 // Lean evaluation of one `column CMP constant` term on a FULL 2048-row (sub-)tile: the comparison runs in the column's
-// own width (one ISETP for <= 4-byte types) and the operator is resolved once per term, not per row.  (ncu on the
-// generic version: 50 instructions per row, issue-bound at 1.6 TB/s on a 4-byte column.)
+// own width (one ISETP for <= 4-byte types) and the operator is resolved once per term, not per row.  (A per-row
+// operator / width dispatch makes the kernel issue-bound on a 4-byte column.)
 template <class T, class CMP>
 __device__ __forceinline__ void eval_rows_lean(const T *p, int tid, T value, bool (&keep)[FT_ROWS], CMP cmp) {
 #pragma unroll
@@ -120,8 +120,8 @@ __device__ __forceinline__ void eval_term_lean(const unsigned char *col, int tid
 // Range form of a term on a full 2048-row sub-tile: ONE subtract and ONE unsigned compare per row whatever the operator
 // (LT / LE / GT / GE / EQ are ranges [lo, hi] of the type's value order, NE the complement; (T)(v - lo) <= (T)(hi - lo)
 // in wrap-around arithmetic of the column's width holds exactly for lo <= v <= hi, signed or unsigned).  Returns bit k
-// = row k * FT_THREADS + tid passes.  (ncu on the switch-per-operator version: 30 instructions per row, issue-bound
-// at 3.2 TB/s on a 4-byte column.)
+// = row k * FT_THREADS + tid passes.  (A switch per operator makes the kernel
+// issue-bound on a 4-byte column.)
 template <class T>
 __device__ __forceinline__ uint32_t range_bits(const unsigned char *col, int tid, uint64_t lo64, uint64_t span64, int neg) {
 	const T *p = (const T *)col;
@@ -247,8 +247,7 @@ __device__ __forceinline__ void mask_single_term(const unsigned char *col, uint6
 }
 
 // A' (two-pass path).  The predicate columns are narrow (a DATE is 4 bytes): a 2048-row tile of one column is 8 KB
-// and the per-tile costs (TMA issue by one thread, mbarrier wait, barriers) dominated - ncu, round 1: 1.45 ms for
-// 2.4 GB.  The mask kernel therefore stages SUPER-tiles of MROWS x 512 rows (up to 16 K rows) and walks them in
+// and the per-tile costs (TMA issue by one thread, mbarrier wait, barriers) dominate.  The mask kernel therefore stages SUPER-tiles of MROWS x 512 rows (up to 16 K rows) and walks them in
 // 2048-row sub-tiles, so that the mask words and the per-2048-row counts keep the layout the scan / compaction expect.
 template <int MROWS>
 __global__ void __launch_bounds__(FT_THREADS) filter_mask_tile_kernel(const __grid_constant__ MaskArgs A) {
@@ -446,8 +445,7 @@ __global__ void __launch_bounds__(FT_THREADS) compact_tile_kernel(const __grid_c
 // where excl(t - G) is the value the SAME CTA computed one iteration earlier (kept in a register).  The G counts are
 // read by the whole CTA in one batch of parallel loads - a wait on publication only, never on another tile's prefix.
 // (A first version used the classic chained look-back: at 2048-row tiles the chain advances ~32 tiles per L2 round
-// trip while HBM delivers ~200 tiles per microsecond; ncu showed the CTAs parked at the barrier behind one spinning
-// thread, 2.1 ms per 128 M rows.)
+// trip, far fewer than HBM delivers, and the CTAs park at the barrier behind one spinning thread.)
 #define FF_PUBLISHED 0x80000000u
 
 struct FusedArgs {
@@ -534,8 +532,7 @@ __device__ __forceinline__ void ff_eval_terms(const FusedArgs &A, const unsigned
 
 // Software-pipelined over the CTA's tiles: iteration k evaluates tile k and publishes its count (phase A), then
 // compacts tile k-1 (phase B), whose prefix needs the counts other CTAs published one phase A ago - by now they are
-// visible, so nobody spins.  (Without the skew every CTA waited every tile for the slowest publication of its round:
-// ncu showed 65 % of the stall samples on that wait, 2.3 ms per 128 M rows.)  Tile k-1's stage and mask stay alive
+// visible, so nobody spins.  (Without the skew every CTA waits every tile for the slowest publication of its round.)  Tile k-1's stage and mask stay alive
 // until its phase B is done; the ring therefore holds S >= 3 stages and refills the stage of tile k-1 with tile
 // k-1+S at the end of iteration k.
 __global__ void __launch_bounds__(FT_THREADS) filter_fused_tile_kernel(const __grid_constant__ FusedArgs A) {

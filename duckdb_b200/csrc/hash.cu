@@ -150,8 +150,7 @@ __global__ void exclusive_scan_small_kernel(const unsigned long long *counts, un
 //                                addresses: stores are coalesced whatever the partition count, and the runs are what
 //                                a peer-memory (NVLink) destination needs.
 // Eligibility: bits <= 4, all columns FLAT without validity, a 2048-row tile of all columns fits 96 KB.
-// (Round 1's versions found a row's rank with one ballot per partition - 16 unrolled ballots per row: 120 and 300
-// instructions per row in ncu, issue-bound at 1.5 TB/s; profiles/r2_part_*.txt.)
+// (One ballot per partition per row - 16 unrolled ballots - makes the kernel issue-bound; match.any replaces them.)
 #define PF_MAXP 16
 #define PF_THREADS 256
 #define PF_ROWS 8
@@ -363,8 +362,7 @@ __global__ void __launch_bounds__(PF_THREADS)
 // The same kernel for the shape the shuffle-join moves (NC 8-byte columns, the BIGINT key among them, column 0 here):
 // ALL global loads of a tile are issued up front into registers (8 rows x NC values per thread), the key is hashed from
 // its register copy instead of being read twice, and the loads complete behind the match / rank / prefix phases.
-// (ncu on the generic version: 42 % of the stall samples on the shared-memory store that waits for the load right in
-// front of it - latency-bound at 3.8 TB/s of DRAM traffic.)
+// (A shared-memory store that waits for the load right in front of it makes the kernel latency-bound.)
 // BULK: every (partition, column) run of the staged tile leaves with ONE bulk-async copy (cp.async.bulk shared -> global,
 // SASS UBLKCP) instead of 8-byte stores - a few large NVLink writes per tile instead of thousands of small ones.  Runs
 // are padded in shared memory so that source and destination share their 16-byte phase; an odd head / tail element

@@ -4,7 +4,7 @@
 // PhysicalHashJoin::{Sink,Finalize,ExecuteInternal} (src/execution/operator/join/physical_hash_join.cpp:764,1893,2140).
 // NULL keys never match (join_hashtable.cpp:714-742); float keys: -0.0 == +0.0, NaN == NaN.
 //
-// Design (B200-first, not the reference's salted pointer table over a row store):
+// Design (GPU-first, not the reference's salted pointer table over a row store):
 //   * build rows live in a COLUMNAR device store (payload columns, flat);
 //   * the hash table is open addressing with 16-byte slots {key64, head_row32, inline32}:
 //       - one key column of <= 8 bytes: key64 is the canonical key itself -> a probe is ONE 32-byte sector,
@@ -746,7 +746,7 @@ int b200_join_probe(b200_join *j, const b200_batch *probe, const int *key_cols, 
 	if (n) {
 		cudaMemsetAsync(j->counters + 1, 0, 8, ctx->stream);
 		// the table is re-used by every probe row: keep (as much as fits of) it in the persisting part of L2
-		// (only worth it when a good part of the table fits: measured on B200, pinning 1/10 of a 1 GiB table is slower)
+		// (only when a good part of the table fits: pinning a small fraction of a large table slows the probe down)
 		if (j->dense && j->dense_range * 4 <= 2 * ctx->l2_persist_max) {
 			b200_l2_pin(ctx, j->dense, j->dense_range * 4);
 		} else if (!j->dense && (j->table_cap + 1) * sizeof(JoinSlot) <= 2 * ctx->l2_persist_max) {

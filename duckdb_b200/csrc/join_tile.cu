@@ -275,7 +275,8 @@ __global__ void __launch_bounds__(JT_THREADS, 2) join_probe_tile_kernel(const __
 					}
 				}
 				if (!knull[k] && !J.build_empty && J.dense) {
-					// direct-addressed table: one 4-byte load, L2-resident for TPC-H sized dimensions
+					// direct-addressed table: one 4-byte load; L2-resident while it fits (50 MB of L2 on an H100 =
+					// ~12 M keys; SF100's 20 M-key part table, 80 MB, is served partly from HBM)
 					uint64_t idx = key[k] - J.dense_min;
 					if (idx < J.dense_range) {
 						uint32_t e = __ldg(&J.dense[idx]);
@@ -419,8 +420,7 @@ __global__ void __launch_bounds__(JT_THREADS, 2) join_probe_tile_kernel(const __
 // without NULLs, payload inline in the table entry or none), written so that nothing is re-derived per row: column
 // offsets, output pointers and payload widths are template / register constants, the four (or eight) table loads of a
 // thread are issued back to back, result positions come from one ballot per row slice and ONE shared-memory atomic
-// per warp per tile.  ncu on the round-1 kernel: 160 instructions per row, issue slots 23 % busy, 2.2 TB/s on a shape
-// whose traffic (42 B/row) allows ~6 TB/s (profiles/r2_join_dense.txt).
+// per warp per tile, so that the kernel is bound by memory rather than by instruction issue.
 template <int NLHS, int ROWS, bool DENSE>
 __global__ void __launch_bounds__(JT_THREADS, 2) join_probe_lean2_kernel(const __grid_constant__ ProbeTileArgs A) {
 	extern __shared__ __align__(128) unsigned char smem_raw[];

@@ -111,7 +111,7 @@ __device__ __forceinline__ void tp_copy_ragged(const TileCols &tc, unsigned char
 }
 
 // Simple (non-specialised) tile loop: every thread is a consumer, thread 0 also issues the TMA copies, one
-// __syncthreads() per tile.  Measured on B200: for kernels whose body already synchronises the CTA per tile (join
+// __syncthreads() per tile.  For kernels whose body already synchronises the CTA per tile (join
 // probe, filter) this is FASTER than the warp-specialised ring below (no 9th warp, no named barriers); the
 // aggregate kernels, whose body never synchronises, use the specialised ring.
 // bars: S mbarriers.  body(stage_ptr, row0, rows_in_tile) is CTA-uniform and may use __syncthreads().

@@ -43,8 +43,8 @@ def exchange_partitions(columns, counts, group=None):
         out.append(o)
     if dev.type == "cuda":
         # The send buffers are views of memory owned by the b200 stream-ordered pool (not by torch's allocator): make
-        # sure NCCL is done with them before the caller frees / reuses that memory.  (Measured on B200 x 2: without
-        # this, back-to-back shuffles raced with the next partition kernel and silently dropped rows.)
+        # sure NCCL is done with them before the caller frees / reuses that memory.  (Without this,
+        # back-to-back shuffles race with the next partition kernel and silently drop rows.)
         torch.cuda.synchronize(dev)
     return out, recv_l
 
@@ -294,8 +294,7 @@ def peer_shuffle_for(ctx, types, rows_hint, group=None):
 
 # ------------------------------------------------------------------------------------------------------------------
 # Shuffle join, pipelined: the probe side is shuffled in chunks on a SECOND stream while the previous chunk is probed on
-# the operator's stream - the NVLink transfer (the bound of the shuffle: (N-1)/N of the probe bytes at ~770 GB/s per
-# GPU) hides behind the probe kernel instead of adding to it.
+# the operator's stream - the NVLink transfer (the bound of the shuffle: (N-1)/N of the probe bytes cross NVLink) hides behind the probe kernel instead of adding to it.
 class PipelinedShuffleProbe:
     """probe(batch, key_cols, lhs_cols, consume): for every chunk of `batch`: peer-shuffle it (double-buffered receive
     buffers, own context + stream, driven by a helper thread) and probe the rows this rank received with `join`

@@ -77,7 +77,7 @@ class Context:
         """stream: None -> the context creates a private non-blocking stream; a CUDA stream handle -> the context
         enqueues on it.  Handle 0 (what torch.cuda.current_stream().cuda_stream returns for torch's default stream)
         is passed on as cudaStreamLegacy (0x1): a NULL handle would mean "create your own" to b200_ctx_create, and
-        the kernels would silently run UNORDERED with torch's / NCCL's work (round 2: rows lost in a 2-GPU shuffle)."""
+        the kernels would silently run UNORDERED with torch's / NCCL's work (rows get lost in a multi-GPU shuffle)."""
         self.handle = C.c_void_p()
         handle = None if stream is None else C.c_void_p(int(stream) if int(stream) != 0 else 1)
         check(lib().b200_ctx_create(device, handle, C.byref(self.handle)))

@@ -1,5 +1,5 @@
 /*
- * duckdb_b200.h - C ABI of the B200-native operator kernels (libduckdb_b200.so).
+ * duckdb_b200.h - C ABI of the H100-native operator kernels (libduckdb_b200.so).
  *
  * This is the drop-in boundary for DuckDB's three hot operator paths.  DuckDB
  * has no C-level physical-operator plugin API (its C API, src/include/duckdb.h,

@@ -111,7 +111,7 @@ public:
 
 //! Probe-side state of one worker: input chunks are buffered (deep copies + their key columns in a pinned staging
 //! buffer) until a batch of B200_PROBE_BATCH rows is full, ONE b200_join_probe call handles the batch, and the result
-//! rows are emitted chunk by chunk (HAVE_MORE_OUTPUT, then FinalExecute for the tail).  A per-chunk probe (round 1) was
+//! rows are emitted chunk by chunk (HAVE_MORE_OUTPUT, then FinalExecute for the tail).  A per-chunk probe would be
 //! one synchronous H2D -> kernel -> D2H round trip per 2048 rows.
 class B200JoinOperatorState : public OperatorState {
 public:

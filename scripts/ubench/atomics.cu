@@ -1,6 +1,6 @@
 // Micro-benchmark: random-access primitives the aggregate / join tables are built from, as a function of the table
-// size (L2-resident vs HBM).  Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o scripts/ubench/_build/atomics
-// scripts/ubench/atomics.cu ; run on a B200: scripts/ubench/_build/atomics [ops_millions]
+// size (L2-resident vs HBM).  Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o scripts/ubench/_build/atomics
+// scripts/ubench/atomics.cu ; run on an H100: scripts/ubench/_build/atomics [ops_millions]
 #include <cuda_runtime.h>
 #include <cstdint>
 #include <cstdio>
@@ -81,7 +81,7 @@ static void run(const char *name, uint64_t *tab, size_t bytes, int stride_words,
 	cudaEvent_t e0, e1;
 	cudaEventCreate(&e0);
 	cudaEventCreate(&e1);
-	int grid = 148 * 8;
+	int grid = 132 * 8; // 8 CTAs per SM of an H100 SXM
 	k<MODE, 4><<<grid, 256>>>(tab, mask, stride_words, n / 4, sink);
 	cudaEventRecord(e0);
 	k<MODE, 4><<<grid, 256>>>(tab, mask, stride_words, n, sink);

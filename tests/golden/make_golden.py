@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
 """Generate the golden fixtures in this directory by running the UNMODIFIED reference
-(oracle/_ref/libduckdb_ref.so, built by oracle/build_ref.py from /root/reference).
+(oracle/_ref/libduckdb_ref.so, built by oracle/build_ref.py from the reference's sources).
 
     python tests/golden/make_golden.py
 
@@ -11,15 +11,23 @@ Outputs (committed):
                    Q14 join (lineitem x part), Q3-shaped join + group-by
   filter_cases.npz random columns + the reference's result for a set of predicates (NULLs, NaN, AND/OR)
   join_cases.npz   random key columns with duplicates/NULLs and the reference's inner/left/semi/anti/mark results
+  reference_results.json  the reference's answers for the tests that compare with it (see reference_results())
+  reference_avg.npz       the reference's avg(d) of every group of test_gpu_parity's group-by, as the exact bit
+                          difference from numpy's bincount mean (mostly 0 to a few units in the last place: the file stays small)
 """
+import json
 import os
+import re
 import sys
 
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))
+from conftest import bincount_mean, digest, digest_array, py_scalar  # noqa: E402
 from oracle import duckdb_ref as R  # noqa: E402
+from oracle.build_ref import REF  # noqa: E402  (DUCKDB_REF: the reference's source tree)
 
 OUT = os.path.dirname(os.path.abspath(__file__))
 rng = np.random.default_rng(42)
@@ -194,15 +202,192 @@ def join_cases(con):
     np.savez_compressed(os.path.join(OUT, "join_cases.npz"), **out)
 
 
+def _enum_values(path, enum_name):
+    """{NAME: value} of `enum class <enum_name>` in a reference header (C rules: previous + 1 when not explicit)."""
+    text = open(os.path.join(REF, path)).read()
+    m = re.search(r"enum class " + enum_name + r"\b[^{]*\{(.*?)\};", text, re.S)
+    assert m, f"{enum_name} not found in {path}"
+    body = re.sub(r"//[^\n]*", "", m.group(1))
+    values, nxt = {}, 0
+    for item in body.split(","):
+        m = re.match(r"\s*([A-Z_0-9]+)\s*(?:=\s*(\d+))?\s*$", item)
+        if not m:
+            continue
+        nxt = int(m.group(2)) if m.group(2) is not None else nxt
+        values[m.group(1)] = nxt
+        nxt += 1
+    return values
+
+
+def _rows(rows):
+    return [[py_scalar(x) for x in r] for r in rows]
+
+
+def _summary(rows):
+    """digest of a sorted row list + its length and first / last rows (they say where a mismatch is)"""
+    rows = list(rows)
+    return {"n": len(rows), "head": _rows(r if isinstance(r, (tuple, list)) else (r,) for r in rows[:3]),
+            "tail": _rows(r if isinstance(r, (tuple, list)) else (r,) for r in rows[-3:]), "sha": digest(rows)}
+
+
+def _column(values):
+    v = np.asarray(values).astype(np.int64)
+    return {"n": len(v), "head": v[:4].tolist(), "sha": digest_array(v)}
+
+
+def reference_results(con):
+    """The reference's answers for the tests that compare with it (tests/test_oracle.py, test_gpu_parity.py,
+    test_gpu_reference_parity.py, test_bench_data.py, test_abi_layout.py).  Each input below is the one the test
+    builds from the same seed or formula; large results are stored as a SHA-256 of their canonical row list
+    (conftest.digest), small ones as rows."""
+    import bench_data as BD
+
+    out = {}
+    # test_oracle.py: hash + group-by
+    rng = np.random.default_rng(7)
+    n = 4000
+    k1 = rng.integers(-3, 3, size=n).astype(np.int32)
+    k1v = rng.random(n) > 0.1
+    k2 = rng.integers(0, 4, size=n).astype(np.uint8)
+    x = rng.integers(-10 ** 12, 10 ** 12, size=n).astype(np.int64)
+    xv = rng.random(n) > 0.2
+    d = rng.standard_normal(n)
+    con.load_table("pg", {"k1": (k1, k1v), "k2": k2, "x": (x, xv), "d": d})
+    h = con.execute("SELECT hash(k1, k2) FROM pg")[0].values
+    con.execute("SET perfect_ht_threshold=0")
+    rows = con.fetchall("SELECT k1, k2, sum(x), count(x), count(*), min(x), max(x), avg(x), sum(d), min(d) "
+                        "FROM pg GROUP BY k1, k2")
+    con.execute("RESET perfect_ht_threshold")
+    out["oracle_groupby"] = {"hash": digest_array(h), "rows": _rows(rows)}
+    # test_oracle.py: joins
+    rng = np.random.default_rng(11)
+    nb, npr = 700, 1500
+    bk = rng.integers(0, 200, size=nb).astype(np.int64)
+    bkv = rng.random(nb) > 0.05
+    bk2 = rng.integers(0, 3, size=nb).astype(np.int16)
+    pk = rng.integers(0, 260, size=npr).astype(np.int64)
+    pkv = rng.random(npr) > 0.05
+    pk2 = rng.integers(0, 3, size=npr).astype(np.int16)
+    con.load_table("jb", {"k": (bk, bkv), "k2": bk2, "id": np.arange(nb, dtype=np.int32)})
+    con.load_table("jp", {"k": (pk, pkv), "k2": pk2, "id": np.arange(npr, dtype=np.int32)})
+    joins = {}
+    for name, keys_sql in (("k", "jp.k = jb.k"), ("k_k2", "jp.k = jb.k AND jp.k2 = jb.k2")):
+        left = con.fetchall(f"SELECT jp.id, jb.id FROM jp LEFT JOIN jb ON {keys_sql}")
+        joins[name] = {
+            "inner": _summary(sorted(con.fetchall(f"SELECT jp.id, jb.id FROM jp JOIN jb ON {keys_sql}"))),
+            "left": _summary(sorted((a, -1 if b is None else b) for a, b in left)),
+            "semi": _summary(sorted(r[0] for r in con.fetchall(f"SELECT jp.id FROM jp SEMI JOIN jb ON {keys_sql}"))),
+            "anti": _summary(sorted(r[0] for r in con.fetchall(f"SELECT jp.id FROM jp ANTI JOIN jb ON {keys_sql}"))),
+        }
+    mark = con.fetchall("SELECT id, k IN (SELECT k FROM jb) FROM jp ORDER BY id")
+    joins["mark"] = _summary([(i, None if m is None else bool(m)) for i, m in mark])
+    fb = np.array([0.0, np.nan, 1.5, -0.0, 2.5], dtype=np.float64)
+    fp = np.array([-0.0, np.nan, 1.5, 7.0, np.nan], dtype=np.float64)
+    con.load_table("fjb", {"k": fb, "id": np.arange(len(fb), dtype=np.int32)})
+    con.load_table("fjp", {"k": fp, "id": np.arange(len(fp), dtype=np.int32)})
+    joins["float_inner"] = _rows(sorted(con.fetchall("SELECT fjp.id, fjb.id FROM fjp JOIN fjb ON fjp.k = fjb.k")))
+    out["oracle_joins"] = joins
+    # test_oracle.py: filters
+    rng = np.random.default_rng(13)
+    n = 3000
+    a = rng.integers(-5, 6, size=n).astype(np.int32)
+    av = rng.random(n) > 0.15
+    b = rng.integers(-5, 6, size=n).astype(np.int32)
+    bv = rng.random(n) > 0.15
+    f = rng.choice(np.array([np.nan, np.inf, -np.inf, -0.0, 0.0, 1.5, -2.25]), size=n)
+    fv = rng.random(n) > 0.1
+    g = rng.choice(np.array([np.nan, np.inf, -0.0, 0.0, 1.5, 3.0]), size=n)
+    con.load_table("fl", {"id": np.arange(n, dtype=np.int32), "a": (a, av), "b": (b, bv), "f": (f, fv), "g": g})
+    sqls = ["a < b", "a = b OR a > 3", "a <> b AND b <= 3", "NOT (a >= b)", "a IS NULL OR b IS NOT NULL",
+            "a IS DISTINCT FROM b", "a IS NOT DISTINCT FROM b", "(a < b) IS NULL", "NOT (a < b AND b < 3) OR a = 3",
+            "f < g", "f >= g", "f = g", "f <> g", "f IS NOT DISTINCT FROM g", "f > 1.5::DOUBLE"]
+    out["oracle_filters"] = {s: _summary(sorted(r[0] for r in con.fetchall(f"SELECT id FROM fl WHERE {s}")))
+                             for s in sqls}
+    # test_gpu_parity.py: group-by + join
+    rng = np.random.default_rng(23)
+    n = 200000
+    k = rng.integers(0, 20000, size=n).astype(np.int64)
+    x = rng.integers(-10 ** 9, 10 ** 9, size=n).astype(np.int64)
+    d = rng.standard_normal(n)
+    con.load_table("lr", {"k": k, "x": x, "d": d})
+    con.execute("SET perfect_ht_threshold=0")
+    rows = sorted(con.fetchall("SELECT k, sum(x), min(x), avg(d), count(*) FROM lr GROUP BY k"))
+    con.execute("RESET perfect_ht_threshold")
+    keys = np.array([r[0] for r in rows], dtype=np.int64)
+    assert np.array_equal(keys, np.unique(k))
+    ref_avg = np.array([r[3] for r in rows], dtype=np.float64)
+    delta = ref_avg.view(np.uint64) - bincount_mean(k, d).view(np.uint64)   # mod 2^64: exact to undo
+    small = delta.view(np.int64)
+    assert np.abs(small).max() < 2 ** 31, "the bincount mean is too far from the reference to store compactly"
+    np.savez_compressed(os.path.join(OUT, "reference_avg.npz"), ulp_delta=small.astype(np.int32))
+    dim = np.unique(k)[::2].astype(np.int64)
+    con.load_table("ld", {"k": dim, "p": (dim * 3).astype(np.int64)})
+    out["gpu_live"] = {
+        "groups": _summary([(r[0], r[1], r[2], r[4]) for r in rows]),
+        "join": _rows([con.fetchall("SELECT count(*), sum(lr.x), sum(ld.p) FROM lr JOIN ld ON lr.k = ld.k")[0]])[0],
+    }
+    # test_gpu_reference_parity.py
+    sf1 = 6_001_215
+    con.execute(BD.q1_table_sql("q1in", sf1))
+    out["sf1_q1"] = _rows(con.fetchall("SELECT rf, ls, sum(qty), sum(price), sum(disc_price), sum(charge), avg(qty), "
+                                       "avg(price), avg(disc), count(*) FROM q1in GROUP BY rf, ls ORDER BY rf, ls"))
+    con.execute("DROP TABLE q1in")
+    con.execute(BD.probe_table_sql("li", sf1, 200_000))
+    con.execute(BD.part_table_sql("part", 200_000))
+    out["sf1_q14"] = _rows([con.fetchall("SELECT count(*), sum(price), sum(disc), sum(promo), sum(li.partkey * promo) "
+                                         "FROM li JOIN part ON li.partkey = part.partkey")[0]])[0]
+    con.execute("DROP TABLE li")
+    con.execute("DROP TABLE part")
+    card = {}
+    for groups, n, keytypes in ((35, 3_000_000, "ssb"), (11_620, 3_000_000, "q3"), (3_500_000, 9_000_000, "q3")):
+        if keytypes == "ssb":
+            con.execute(BD.ssb_table_sql("t", n))
+            sql = "SELECT year, nation, sum(profit), count(*) FROM t GROUP BY year, nation"
+        else:
+            con.execute(BD.q3_table_sql("t", n, groups))
+            sql = "SELECT okey, odate, prio, sum(revenue), count(*) FROM t GROUP BY okey, odate, prio"
+        rows = con.fetchall(sql)
+        card[f"{keytypes}_{groups}_{n}"] = _summary(sorted(rows))
+        con.execute("DROP TABLE t")
+    out["sf1_groupby"] = card
+    # test_bench_data.py: the synthetic columns as the reference's SQL defines them
+    bench = {}
+
+    def columns(sql):
+        con.execute("DROP TABLE IF EXISTS t")
+        con.execute(sql)
+        return {c.name: _column(c.values) for c in con.execute("SELECT * FROM t")}
+
+    for offset in (0, 591_855_000 * 3 + 12345):
+        bench[f"q1_{offset}"] = columns(BD.q1_table_sql("t", 50_000, offset))
+    n, nb, groups = 40_000, 1000, 5000
+    bench["ssb"] = columns(BD.ssb_table_sql("t", n, 77))
+    bench["q3"] = columns(BD.q3_table_sql("t", n, groups, 5))
+    bench["probe"] = columns(BD.probe_table_sql("t", n, nb, 3))
+    bench["part"] = columns(BD.part_table_sql("t", nb, 1001))
+    bench["scan"] = columns(BD.scan_table_sql("t", n, 9))
+    con.execute("DROP TABLE t")
+    out["bench_data"] = bench
+    # test_abi_layout.py: DuckDB's enum values the C ABI reuses
+    out["enums"] = {
+        "PhysicalType": _enum_values("src/include/duckdb/common/types.hpp", "PhysicalType"),
+        "ExpressionType": _enum_values("src/include/duckdb/common/enums/expression_type.hpp", "ExpressionType"),
+        "JoinType": _enum_values("src/include/duckdb/common/enums/join_type.hpp", "JoinType"),
+        "VectorType": _enum_values("src/include/duckdb/common/enums/vector_type.hpp", "VectorType"),
+    }
+    with open(os.path.join(OUT, "reference_results.json"), "w") as fh:
+        json.dump(out, fh, sort_keys=True, separators=(",", ":"))
+        fh.write("\n")
+
+
 def main():
+    """With arguments: only the named fixtures (e.g. `reference_results`), so that the others are not rewritten."""
     con = R.Connection(threads=4)
-    hash_kat(con)
-    filter_cases(con)
-    join_cases(con)
-    tpch(con)
+    for fn in sys.argv[1:] or ["hash_kat", "filter_cases", "join_cases", "tpch", "reference_results"]:
+        globals()[fn](con)
     con.close()
     for f in sorted(os.listdir(OUT)):
-        if f.endswith(".npz"):
+        if f.endswith((".npz", ".json")):
             print(f, os.path.getsize(os.path.join(OUT, f)))
 
 

@@ -27,7 +27,7 @@ def test_library_exports_every_declared_symbol():
 
 def test_version_and_error_strings():
     L = capi.lib()
-    assert b"sm_100a" in L.b200_version()
+    assert b"sm_90a" in L.b200_version()
     assert isinstance(L.b200_last_error(), bytes)
 
 

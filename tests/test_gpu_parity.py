@@ -1,10 +1,10 @@
-"""Parity of the CUDA path (through the C ABI) with the oracle, the golden fixtures of the unmodified
-reference, and - when oracle/_ref travelled to this box - the live reference.  Integer results bit-exact;
+"""Parity of the CUDA path (through the C ABI) with the oracle and the golden fixtures of the unmodified
+reference.  Integer results bit-exact;
 double SUM/AVG within 1e-9 relative (BASELINE.json north_star)."""
 import numpy as np
 import pytest
 
-from conftest import golden
+from conftest import assert_matches, bincount_mean, golden
 from duckdb_b200 import capi
 from duckdb_b200 import operators as ops
 from oracle import port as P
@@ -777,29 +777,25 @@ def test_partition_scatter_dev_capacity_guard(ctx, bulk, tight, monkeypatch):
     assert int(dropped.item()) == expect_dropped
 
 
-# ------------------------------------------------------------------ live reference (when oracle/_ref travelled)
-@pytest.mark.ref
-def test_live_reference_groupby_and_join(ctx, refcon):
+# ------------------------------------------------------------------ the reference's answers (tests/golden/reference_results.json)
+def test_live_reference_groupby_and_join(ctx, reference_results):
+    ref = reference_results["gpu_live"]
     rng = np.random.default_rng(23)
     n = 200000
     k = rng.integers(0, 20000, size=n).astype(np.int64)
     x = rng.integers(-10 ** 9, 10 ** 9, size=n).astype(np.int64)
     d = rng.standard_normal(n)
-    refcon.execute("DROP TABLE IF EXISTS lr")
-    refcon.load_table("lr", {"k": k, "x": x, "d": d})
-    refcon.execute("SET perfect_ht_threshold=0")
-    rows = refcon.fetchall("SELECT k, sum(x), min(x), avg(d), count(*) FROM lr GROUP BY k")
+    # SELECT k, sum(x), min(x), avg(d), count(*) FROM lr GROUP BY k
     aggs = [("sum", (x, None)), ("min", (x, None)), ("avg", (d, None)), ("count_star", None)]
     got = run_agg(ctx, [(k, None)], aggs, n, batches=2)
-    assert len(got) == len(rows)
-    for r in rows:
-        gv = got[(r[0],)]
-        assert gv[0] == r[1] and gv[1] == r[2] and gv[3] == r[4]
-        assert gv[2] == pytest.approx(r[3], rel=1e-9, abs=1e-12)
+    assert_matches(sorted((key[0], gv[0], gv[1], gv[3]) for key, gv in got.items()), ref["groups"], "sum/min/count")
+    # the reference's avg(d) of every group, rebuilt bit for bit from numpy's mean and the stored difference
+    ref_avg = (bincount_mean(k, d).view(np.uint64) + golden("reference_avg.npz")["ulp_delta"].astype(np.int64).view(np.uint64)
+               ).view(np.float64)
+    for key, avg in zip(np.unique(k).tolist(), ref_avg.tolist()):
+        assert got[(key,)][2] == pytest.approx(avg, rel=1e-9, abs=1e-12), key
     dim = np.unique(k)[::2].astype(np.int64)
-    refcon.execute("DROP TABLE IF EXISTS ld")
-    refcon.load_table("ld", {"k": dim, "p": (dim * 3).astype(np.int64)})
-    cnt, sx, sp = refcon.fetchall("SELECT count(*), sum(lr.x), sum(ld.p) FROM lr JOIN ld ON lr.k = ld.k")[0]
+    cnt, sx, sp = ref["join"]   # SELECT count(*), sum(lr.x), sum(ld.p) FROM lr JOIN ld ON lr.k = ld.k
     res, _, count = run_join(ctx, "inner", [(dim, None)], [((dim * 3).astype(np.int64), None)], [(k, None)],
                              [(x, None)], len(dim), n)
     assert count == cnt

@@ -1,9 +1,9 @@
-"""The CPU oracle (oracle/port.py) pinned against the reference's own known-answer vectors, the golden
-fixtures generated from the unmodified reference, and (when present) the live reference library."""
+"""The CPU oracle (oracle/port.py) pinned against the reference's own known-answer vectors and the golden
+fixtures generated from the unmodified reference."""
 import numpy as np
 import pytest
 
-from conftest import golden
+from conftest import assert_matches, digest_array, golden
 from oracle import port as P
 
 
@@ -146,8 +146,10 @@ def test_radix_partition_ids():
     np.testing.assert_array_equal(P.radix_partition_ids(h, 0), [0, 0, 0, 0, 0])
 
 
-@pytest.mark.ref
-def test_port_vs_live_reference_hash_and_groupby(refcon):
+def test_port_vs_live_reference_hash_and_groupby(reference_results):
+    """hash() and a group-by with NULL keys / NULL inputs of the port against the reference's answers on the same
+    seeded rows (tests/golden/reference_results.json)."""
+    ref = reference_results["oracle_groupby"]
     rng = np.random.default_rng(7)
     n = 4000
     k1 = rng.integers(-3, 3, size=n).astype(np.int32)
@@ -156,13 +158,8 @@ def test_port_vs_live_reference_hash_and_groupby(refcon):
     x = rng.integers(-10 ** 12, 10 ** 12, size=n).astype(np.int64)
     xv = rng.random(n) > 0.2
     d = rng.standard_normal(n)
-    refcon.execute("DROP TABLE IF EXISTS pg")
-    refcon.load_table("pg", {"k1": (k1, k1v), "k2": k2, "x": (x, xv), "d": d})
-    h = refcon.execute("SELECT hash(k1, k2) FROM pg")[0].values
-    np.testing.assert_array_equal(P.hash_columns([(k1, k1v), (k2, None)]), h)
-    refcon.execute("SET perfect_ht_threshold=0")
-    rows = refcon.fetchall("SELECT k1, k2, sum(x), count(x), count(*), min(x), max(x), avg(x), sum(d), min(d) "
-                           "FROM pg GROUP BY k1, k2")
+    assert digest_array(P.hash_columns([(k1, k1v), (k2, None)])) == ref["hash"]
+    rows = ref["rows"]
     res = P.group_by([(k1, k1v), (k2, None)],
                      [("sum", (x, xv)), ("count", (x, xv)), ("count_star", None), ("min", (x, xv)),
                       ("max", (x, xv)), ("avg", (x, xv)), ("sum", (d, None)), ("min", (d, None))], n)
@@ -175,10 +172,10 @@ def test_port_vs_live_reference_hash_and_groupby(refcon):
         assert got[7] == r[9]
 
 
-@pytest.mark.ref
-def test_port_vs_live_reference_joins(refcon):
-    """every join type of the port against the unmodified reference: NULL keys on both sides, duplicate build
+def test_port_vs_live_reference_joins(reference_results):
+    """every join type of the port against the reference's answers: NULL keys on both sides, duplicate build
     keys, composite keys, float keys with NaN / -0.0."""
+    ref = reference_results["oracle_joins"]
     rng = np.random.default_rng(11)
     nb, npr = 700, 1500
     bk = rng.integers(0, 200, size=nb).astype(np.int64)
@@ -187,40 +184,24 @@ def test_port_vs_live_reference_joins(refcon):
     pk = rng.integers(0, 260, size=npr).astype(np.int64)
     pkv = rng.random(npr) > 0.05
     pk2 = rng.integers(0, 3, size=npr).astype(np.int16)
-    for t in ("jb", "jp"):
-        refcon.execute(f"DROP TABLE IF EXISTS {t}")
-    refcon.load_table("jb", {"k": (bk, bkv), "k2": bk2, "id": np.arange(nb, dtype=np.int32)})
-    refcon.load_table("jp", {"k": (pk, pkv), "k2": pk2, "id": np.arange(npr, dtype=np.int32)})
-    for keys_sql, bkeys, pkeys in [("jp.k = jb.k", [(bk, bkv)], [(pk, pkv)]),
-                                   ("jp.k = jb.k AND jp.k2 = jb.k2", [(bk, bkv), (bk2, None)], [(pk, pkv), (pk2, None)])]:
-        inner = refcon.fetchall(f"SELECT jp.id, jb.id FROM jp JOIN jb ON {keys_sql}")
-        assert sorted(inner) == P.hash_join(bkeys, pkeys, nb, npr, "inner")
-        left = refcon.fetchall(f"SELECT jp.id, jb.id FROM jp LEFT JOIN jb ON {keys_sql}")
-        assert sorted((a, -1 if b is None else b) for a, b in left) == P.hash_join(bkeys, pkeys, nb, npr, "left")
-        semi = refcon.fetchall(f"SELECT jp.id FROM jp SEMI JOIN jb ON {keys_sql}")
-        assert sorted(r[0] for r in semi) == P.hash_join(bkeys, pkeys, nb, npr, "semi")
-        anti = refcon.fetchall(f"SELECT jp.id FROM jp ANTI JOIN jb ON {keys_sql}")
-        assert sorted(r[0] for r in anti) == P.hash_join(bkeys, pkeys, nb, npr, "anti")
+    for name, bkeys, pkeys in [("k", [(bk, bkv)], [(pk, pkv)]),
+                               ("k_k2", [(bk, bkv), (bk2, None)], [(pk, pkv), (pk2, None)])]:
+        for how in ("inner", "left", "semi", "anti"):
+            assert_matches(P.hash_join(bkeys, pkeys, nb, npr, how), ref[name][how], (name, how))
     # MARK join = `k IN (subquery)` in the select list: TRUE / FALSE / NULL per probe row
-    mark = refcon.fetchall("SELECT id, k IN (SELECT k FROM jb) FROM jp ORDER BY id")
     matched, valid = P.hash_join([(bk, bkv)], [(pk, pkv)], nb, npr, "mark")
-    for (_, m), pm, pv in zip(mark, matched, valid):
-        assert (m is None) == (not pv) and (m is None or bool(m) == bool(pm))
+    assert_matches([(i, bool(m) if v else None) for i, (m, v) in enumerate(zip(matched, valid))], ref["mark"], "mark")
     # float keys: NaN joins NaN, -0.0 joins +0.0 (comparison_operators.cpp:24-40)
     fb = np.array([0.0, np.nan, 1.5, -0.0, 2.5], dtype=np.float64)
     fp = np.array([-0.0, np.nan, 1.5, 7.0, np.nan], dtype=np.float64)
-    for t in ("fjb", "fjp"):
-        refcon.execute(f"DROP TABLE IF EXISTS {t}")
-    refcon.load_table("fjb", {"k": fb, "id": np.arange(len(fb), dtype=np.int32)})
-    refcon.load_table("fjp", {"k": fp, "id": np.arange(len(fp), dtype=np.int32)})
-    got = refcon.fetchall("SELECT fjp.id, fjb.id FROM fjp JOIN fjb ON fjp.k = fjb.k")
-    assert sorted(got) == P.hash_join([(fb, None)], [(fp, None)], len(fb), len(fp), "inner")
+    got = P.hash_join([(fb, None)], [(fp, None)], len(fb), len(fp), "inner")
+    assert [list(r) for r in got] == ref["float_inner"]
 
 
-@pytest.mark.ref
-def test_port_vs_live_reference_filters(refcon):
+def test_port_vs_live_reference_filters(reference_results):
     """three-valued logic, NULL comparisons, IS [NOT] DISTINCT FROM and the float total order of the port against
     the reference's WHERE clause, on random data with NULLs / NaN / infinities."""
+    ref = reference_results["oracle_filters"]
     rng = np.random.default_rng(13)
     n = 3000
     a = rng.integers(-5, 6, size=n).astype(np.int32)
@@ -230,8 +211,6 @@ def test_port_vs_live_reference_filters(refcon):
     f = rng.choice(np.array([np.nan, np.inf, -np.inf, -0.0, 0.0, 1.5, -2.25]), size=n)
     fv = rng.random(n) > 0.1
     g = rng.choice(np.array([np.nan, np.inf, -0.0, 0.0, 1.5, 3.0]), size=n)
-    refcon.execute("DROP TABLE IF EXISTS fl")
-    refcon.load_table("fl", {"id": np.arange(n, dtype=np.int32), "a": (a, av), "b": (b, bv), "f": (f, fv), "g": g})
     cols = [(a, av), (b, bv), (f, fv), (g, None)]
     A, B, F, G = ("col", 0), ("col", 1), ("col", 2), ("col", 3)
     c3 = ("const", 3, np.int32)
@@ -252,10 +231,10 @@ def test_port_vs_live_reference_filters(refcon):
         "f IS NOT DISTINCT FROM g": ("notdistinct", F, G),
         "f > 1.5::DOUBLE": ("gt", F, ("const", 1.5, np.float64)),
     }
+    assert set(cases) == set(ref)
     for sql, tree in cases.items():
-        exp = sorted(r[0] for r in refcon.fetchall(f"SELECT id FROM fl WHERE {sql}"))
         sel, _ = P.filter_select(tree, cols, n)
-        assert sel.tolist() == exp, sql
+        assert_matches(sel.tolist(), ref[sql], sql)
 
 
 def test_aggregate_kats_from_reference_tests():
