@@ -562,6 +562,28 @@ extern "C" int b200_filter_project(b200_ctx *ctx, const b200_batch *in, const b2
 			b200_set_error("b200_filter_project: node %d has unsupported type %d", i, nd.type);
 			return B200_ERR_INVALID;
 		}
+		// Both operands of a comparison have one type (DuckDB binds them so) and an integer constant holds a value of
+		// its type: the interpreter compares in the left operand's type, the tile path in the column's, and the two
+		// only agree under these rules.
+		if ((nd.op >= B200_EXPR_EQ && nd.op <= B200_EXPR_GE) || nd.op == B200_EXPR_DISTINCT ||
+		    nd.op == B200_EXPR_NOT_DISTINCT) {
+			if (nodes[nd.left].type != nodes[nd.right].type) {
+				b200_set_error("b200_filter_project: node %d compares type %d with type %d", i, nodes[nd.left].type,
+				               nodes[nd.right].type);
+				return B200_ERR_INVALID;
+			}
+		}
+		if (nd.op == B200_EXPR_CONST && !nd.is_null && b200_type_is_integer(nd.type) && b200_type_size(nd.type) < 8) {
+			const int bits = b200_type_size(nd.type) * 8;
+			const int64_t v = nd.value.i;
+			bool ok = b200_type_is_signed_int(nd.type) ? (v >= -(1LL << (bits - 1)) && v < (1LL << (bits - 1)))
+			                                           : (v >= 0 && v < (1LL << bits));
+			if (!ok) {
+				b200_set_error("b200_filter_project: constant node %d holds %lld, outside its type %d", i, (long long)v,
+				               nd.type);
+				return B200_ERR_INVALID;
+			}
+		}
 		if (nd.op == B200_EXPR_COLREF) {
 			if (nd.col < 0 || nd.col >= (int)in->cols.size() || nd.col >= 256) {
 				b200_set_error("b200_filter_project: node %d references column %d (batch has %d)", i, nd.col,

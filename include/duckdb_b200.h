@@ -189,8 +189,10 @@ typedef struct b200_expr_node {
 		uint64_t u;
 		double d;
 		float f;
-	} value;          /* CONST payload */
+	} value;          /* CONST payload; an integer constant must be representable in `type` */
 } b200_expr_node;
+/* The two operands of a comparison (EQ .. GE, DISTINCT, NOT_DISTINCT) must have the same type;
+ * b200_filter_project returns B200_ERR_INVALID otherwise. */
 
 /* One pass of PhysicalFilter (+ the PhysicalProjection above it):
  *   rows for which node `filter_root` is TRUE (not NULL, not false) survive

@@ -1,0 +1,62 @@
+"""Every __global__ kernel of the fast-path sources is claimed by a case of tests/test_gpu_kernel_paths.py (which asserts,
+through the kernel trace, that it ran) or excluded there with a reason: a new kernel variant fails this test until a
+GPU case covers it."""
+import ast
+import os
+import re
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+CSRC = os.path.join(ROOT, "duckdb_b200", "csrc")
+SOURCES = ["filter_tile.cu", "agg_hc.cu", "join_tile.cu"]
+GPU_MODULE = os.path.join(ROOT, "tests", "test_gpu_kernel_paths.py")
+
+_GLOBAL = re.compile(r"__global__\s+void\s+(?:__launch_bounds__\s*\([^()]*\)\s*)?(\w+)\s*\(")
+
+
+def kernels_in(path):
+    with open(path) as f:
+        text = re.sub(r"//[^\n]*", "", f.read())
+    return set(_GLOBAL.findall(text))
+
+
+def gpu_module():
+    with open(GPU_MODULE) as f:
+        source = f.read()
+    tree = ast.parse(source)
+    consts, funcs = {}, {}
+    for node in tree.body:
+        if isinstance(node, ast.Assign) and len(node.targets) == 1 and isinstance(node.targets[0], ast.Name) and \
+                node.targets[0].id in ("KERNEL_CASES", "KERNEL_EXCLUDED"):
+            consts[node.targets[0].id] = ast.literal_eval(node.value)
+        elif isinstance(node, ast.FunctionDef):
+            funcs[node.name] = ast.get_source_segment(source, node)
+    return consts["KERNEL_CASES"], consts["KERNEL_EXCLUDED"], funcs
+
+
+def test_parser_finds_the_known_kernels():
+    found = set().union(*(kernels_in(os.path.join(CSRC, s)) for s in SOURCES))
+    for k in ["filter_mask_tile_kernel", "compact_tile_kernel", "filter_fused_tile_kernel", "agg_hc_kernel",
+              "agg_hc_simple_kernel", "agg_hc_direct_kernel", "join_probe_tile_kernel", "join_probe_lean2_kernel"]:
+        assert k in found, k
+
+
+def test_every_fast_path_kernel_has_a_gpu_case():
+    cases, excluded, _ = gpu_module()
+    for src in SOURCES:
+        for k in sorted(kernels_in(os.path.join(CSRC, src))):
+            assert k in cases or k in excluded, \
+                f"{src}: kernel {k} has no case in KERNEL_CASES of test_gpu_kernel_paths.py and no exclusion"
+            if k in excluded:
+                assert isinstance(excluded[k], str) and excluded[k].strip(), f"{k}: an exclusion needs a reason"
+
+
+def test_kernel_cases_name_tests_that_check_the_kernel():
+    cases, excluded, funcs = gpu_module()
+    known = set().union(*(kernels_in(os.path.join(CSRC, s)) for s in SOURCES))
+    for k, tests in cases.items():
+        assert k in known, f"KERNEL_CASES lists {k}, which no longer exists"
+        assert k not in excluded, k
+        assert tests, k
+        for t in tests:
+            assert t.startswith("test_") and t in funcs, f"{k}: no test function {t}"
+            assert k in funcs[t], f"{t} does not name {k}: it cannot be asserting that the kernel ran"
