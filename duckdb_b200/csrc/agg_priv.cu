@@ -9,8 +9,9 @@
 // table with one atomic per (CTA, group, state), exactly like FAST / FASTREG.
 //
 // Eligibility (same as FASTREG): integer group keys without NULLs packed in <= 7 bytes, every aggregate is
-// sum / avg / count over non-NULL 8-byte integers.  Values with |x| >= 2^40 and keys beyond the CTA's slots take the
-// global path inline (row_to_global) and are counted in counters[1].
+// sum / avg / count over non-NULL 8-byte integers.  Values outside [-2^40, 2^40) (unsigned: >= 2^40, see
+// reg_value_too_big) and keys beyond the CTA's slots take the global path inline (row_to_global); rows whose key missed
+// are counted in counters[1].
 // Reference semantics: GroupedAggregateHashTable::FindOrCreateGroupsInternal + UpdateAggregates
 // (src/execution/aggregate_hashtable.cpp:803-977,688-722), integer sums as hugeint (sum_helpers.hpp:155-215).
 #include "agg_tile.cuh"
@@ -210,7 +211,7 @@ __global__ void __launch_bounds__(512 + 32, 1)
 				uint64_t big = 0;
 #pragma unroll
 				for (int j = 0; j < NSUM; j++) {
-					big |= (x[k][j] + (1ULL << 40)) >> 41;
+					big |= reg_value_too_big(x[k][j], (R.sum_unsigned >> j) & 1);
 				}
 				if (KW != 2) {
 					slot[k] = -1;
@@ -292,7 +293,7 @@ __global__ void __launch_bounds__(512 + 32, 1)
 				for (int t = lane; t < NC; t += 32) {
 					uint64_t v = acc[((size_t)s * NSUM + j) * NC + t];
 					uint64_t nl = lo + v;
-					hi += ((int64_t)v < 0 ? ~0ULL : 0ULL) + (nl < lo ? 1 : 0); // partials are signed 64-bit (|.| < 2^62)
+					hi += ((int64_t)v < 0 ? ~0ULL : 0ULL) + (nl < lo ? 1 : 0); // partials are signed 64-bit (reg_value_too_big)
 					lo = nl;
 				}
 				for (int off = 16; off; off >>= 1) {
@@ -391,7 +392,7 @@ __global__ void __launch_bounds__(512 + 32, 1)
 #pragma unroll
 				for (int j = 0; j < NSUM; j++) {
 					x[k][j] = *(const uint64_t *)(stage + R.sum_smem_off[j] + (size_t)r * 8);
-					big |= (x[k][j] + (1ULL << 40)) >> 41;
+					big |= reg_value_too_big(x[k][j], (R.sum_unsigned >> j) & 1);
 				}
 				slot[k] = ok[k] && !big ? sl[k] : -1;
 				if (live && slot[k] < 0) {
@@ -455,7 +456,7 @@ __global__ void __launch_bounds__(512 + 32, 1)
 #pragma unroll
 			for (int j = 0; j < NSUM; j++) {
 				uint64_t lo = lane < nwarps ? acc[((size_t)lane * SLOTS + s) * NSUM + j] : 0;
-				uint64_t hi = (int64_t)lo < 0 ? ~0ULL : 0ULL; // partials are signed 64-bit values (|.| < 2^62)
+				uint64_t hi = (int64_t)lo < 0 ? ~0ULL : 0ULL; // partials are signed 64-bit values (reg_value_too_big)
 				for (int off = 16; off; off >>= 1) {
 					uint64_t olo = __shfl_xor_sync(0xffffffffu, lo, off);
 					uint64_t ohi = __shfl_xor_sync(0xffffffffu, hi, off);
@@ -610,6 +611,7 @@ int b200_agg_priv_launch(b200_ctx *ctx, TileArgs &A, const AggLayout &L, const K
 			if (R.nsum >= REG_MAX_SUMS || b200_type_size(L.input_type[i]) != 8) {
 				return B200_ERR_INVALID;
 			}
+			R.sum_unsigned |= (b200_type_is_unsigned_int(L.input_type[i]) ? 1u : 0u) << R.nsum;
 			R.in_of_sum[R.nsum++] = i;
 		}
 	}

@@ -255,8 +255,8 @@ __global__ void __launch_bounds__(AT_THREADS + 32) agg_fast_kernel(const __grid_
 // NULLs, every aggregate is sum / avg / count over NON-NULL 8-byte integer inputs (BIGINT / DECIMAL(<=18)).
 // The per-thread partial sums live in REGISTERS (acc[slot][sum]); a row adds each value to every slot under a
 // predicate (hit[slot]) - no shared-memory traffic for the states, no atomics, and the predicated adds are
-// independent, so the SM issues them back to back.  Values with |x| >= 2^40 (whose per-thread partial could
-// overflow 64 bits) take the global path.
+// independent, so the SM issues them back to back.  Values outside [-2^40, 2^40) for a signed input, or >= 2^40
+// for an unsigned one (whose per-thread partial could overflow the signed 64-bit range), take the global path.
 // acc[j] += x[j] for all j, rows += 1, under one predicate.  Written on the 32-bit halves so that ptxas keeps
 // the low add predicated (3 SASS instructions per 64-bit accumulate instead of add + 2 selects).
 __device__ __forceinline__ void pred_add64(uint64_t &acc, uint64_t x, uint32_t hit) {
@@ -335,7 +335,7 @@ __global__ void __launch_bounds__(THREADS + 32, 2) agg_fastreg_kernel(const __gr
 #pragma unroll
 		for (int j = 0; j < NSUM; j++) {
 			x[j] = *(const uint64_t *)(stage + R.sum_smem_off[j] + (size_t)r * 8);
-			big |= (x[j] + (1ULL << 40)) >> 41;
+			big |= reg_value_too_big(x[j], (R.sum_unsigned >> j) & 1);
 		}
 		if (!any || big) {
 			// slow path: first time this thread sees the key (look it up / insert it in the CTA's directory),
@@ -392,7 +392,7 @@ __global__ void __launch_bounds__(THREADS + 32, 2) agg_fastreg_kernel(const __gr
 #pragma unroll
 		for (int j = 0; j < NSUM; j++) {
 			uint64_t lo = acc[s][j];
-			uint64_t hi = (int64_t)lo < 0 ? ~0ULL : 0ULL; // partials are signed 64-bit values (|.| < 2^62)
+			uint64_t hi = (int64_t)lo < 0 ? ~0ULL : 0ULL; // partials are signed 64-bit values (reg_value_too_big)
 			for (int off = 16; off; off >>= 1) {
 				uint64_t olo = __shfl_xor_sync(0xffffffffu, lo, off);
 				uint64_t ohi = __shfl_xor_sync(0xffffffffu, hi, off);
@@ -662,7 +662,7 @@ __global__ void __launch_bounds__(AT_THREADS + 32) agg_mid_kernel(const __grid_c
 // fire-and-forget shared-memory RED (no return value, no carry chain).  A word absorbs 2^18 additions of a
 // 14-bit limb before it could wrap, so the CTA flushes its table into the global table every 2^18 rows
 // (flush_tiles tiles) and at the end: sum = w0 + (w1 << 14) + (w2 << 28) - count * 2^40.
-// Rows with a value outside +-2^40 take the global path (like the register fast path).  More consumer warps than
+// Rows with a value outside [-2^40, 2^40) (unsigned: >= 2^40) take the global path (like the register fast path).  More consumer warps than
 // MID (the slot lookup is a chain of dependent shared-memory loads; the REDs are not waited for).
 // NOT yet measured on hardware: off by default, see DESIGN.md section 8.
 struct Mid2Layout {
@@ -867,8 +867,11 @@ __global__ void __launch_bounds__(NC + 32, 1) agg_mid2_kernel(const __grid_const
 #pragma unroll 1
 		    for (int i = 0; i < L.ninputs; i++) {
 			    if (M.w_sum[i] >= 0 && stage_valid(stage, A.tc, A.sm.in_valid[i], r)) {
-				    int64_t v = (int64_t)stage_value(stage, A.tc.c[A.sm.in_data[i]], L.input_type[i], r);
-				    in_range = in_range && (uint64_t)(v + (1LL << MID2_BIAS_SHIFT)) < (1ULL << (MID2_BIAS_SHIFT + 1));
+				    uint64_t raw = stage_value(stage, A.tc.c[A.sm.in_data[i]], L.input_type[i], r);
+				    // unsigned: raw < 2^40 (a UBIGINT >= 2^63 read as int64 would look small and negative)
+				    in_range = in_range && (b200_type_is_unsigned_int(L.input_type[i])
+				                                ? raw < (1ULL << MID2_BIAS_SHIFT)
+				                                : raw + (1ULL << MID2_BIAS_SHIFT) < (1ULL << (MID2_BIAS_SHIFT + 1)));
 			    }
 		    }
 		    if (!in_range) {
@@ -1047,6 +1050,7 @@ int b200_agg_tile_sink(b200_ctx *ctx, int mode, int slots_hint, const AggLayout 
 					reg_ok = false;
 				} else {
 					R.sum_smem_off[R.nsum] = A.tc.c[A.sm.in_data[i]].smem_off;
+					R.sum_unsigned |= (b200_type_is_unsigned_int(L.input_type[i]) ? 1u : 0u) << R.nsum;
 					R.in_of_sum[R.nsum++] = i;
 				}
 			}

@@ -168,11 +168,24 @@ struct RegLayout {
 	int nsum;
 	int in_of_sum[REG_MAX_SUMS];         // distinct-input index of sum accumulator j
 	uint32_t sum_smem_off[REG_MAX_SUMS]; // byte offset of the input's tile inside a stage
+	uint32_t sum_unsigned;               // bit j: the input of sum accumulator j is an unsigned integer
 	int nkeys;
 	uint32_t key_smem_off[MAX_KEYS];
 	uint32_t key_width[MAX_KEYS]; // 1, 2, 4 or 8 bytes
 	uint32_t key_shift[MAX_KEYS]; // bit position inside the (single) packed key word
 };
+
+// Non-zero when the 8-byte integer x is too large for the 64-bit per-thread partials of FASTREG / PRIV / WPRIV and
+// must take the global path: x outside [-2^40, 2^40) for a signed input, x >= 2^40 for an unsigned one.  The signed
+// test alone, (x + 2^40) >> 41, would let an unsigned x >= 2^64 - 2^40 wrap to a small value and stay.  Both tests
+// only read the high word (adding 2^40 leaves the low word alone): signed (hi + 2^8) >> 9, unsigned hi >> 8.
+// With them, a partial of k kept values lies in (-k 2^40, k 2^40), inside the signed 64-bit range for k < 2^23, so
+// the reductions may widen every partial as a SIGNED 64-bit value, unsigned inputs included.
+__device__ __forceinline__ uint32_t reg_value_too_big(uint64_t x, bool is_unsigned) {
+	const uint32_t bias = is_unsigned ? 0u : 1u << 8;
+	const uint32_t mask = is_unsigned ? ~0xffu : ~0x1ffu;
+	return ((uint32_t)(x >> 32) + bias) & mask;
+}
 
 // zero-extended load of a 1/2/4/8-byte integer from a staged tile
 __device__ __forceinline__ uint64_t stage_load_uint(const unsigned char *p, uint32_t width) {

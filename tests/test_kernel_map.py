@@ -1,14 +1,17 @@
-"""Every __global__ kernel of the fast-path sources is claimed by a case of tests/test_gpu_kernel_paths.py (which asserts,
-through the kernel trace, that it ran) or excluded there with a reason: a new kernel variant fails this test until a
-GPU case covers it."""
+"""Every __global__ kernel of the fast-path and aggregate sources is claimed by a case of the GPU module that owns the
+source (which asserts, through the kernel trace, that it ran) or excluded there with a reason: a new kernel variant
+fails this test until a GPU case covers it."""
 import ast
 import os
 import re
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "duckdb_b200", "csrc")
-SOURCES = ["filter_tile.cu", "agg_hc.cu", "join_tile.cu"]
-GPU_MODULE = os.path.join(ROOT, "tests", "test_gpu_kernel_paths.py")
+# GPU test module -> the sources whose kernels its KERNEL_CASES / KERNEL_EXCLUDED must account for
+MODULES = {
+    "test_gpu_kernel_paths.py": ["filter_tile.cu", "agg_hc.cu", "join_tile.cu"],
+    "test_gpu_agg_kernel_paths.py": ["agg_tile.cu", "agg_priv.cu", "agg.cu"],
+}
 
 _GLOBAL = re.compile(r"__global__\s+void\s+(?:__launch_bounds__\s*\([^()]*\)\s*)?(\w+)\s*\(")
 
@@ -19,8 +22,8 @@ def kernels_in(path):
     return set(_GLOBAL.findall(text))
 
 
-def gpu_module():
-    with open(GPU_MODULE) as f:
+def gpu_module(name):
+    with open(os.path.join(ROOT, "tests", name)) as f:
         source = f.read()
     tree = ast.parse(source)
     consts, funcs = {}, {}
@@ -34,29 +37,44 @@ def gpu_module():
 
 
 def test_parser_finds_the_known_kernels():
-    found = set().union(*(kernels_in(os.path.join(CSRC, s)) for s in SOURCES))
+    found = set().union(*(kernels_in(os.path.join(CSRC, s)) for srcs in MODULES.values() for s in srcs))
     for k in ["filter_mask_tile_kernel", "compact_tile_kernel", "filter_fused_tile_kernel", "agg_hc_kernel",
-              "agg_hc_simple_kernel", "agg_hc_direct_kernel", "join_probe_tile_kernel", "join_probe_lean2_kernel"]:
+              "agg_hc_simple_kernel", "agg_hc_direct_kernel", "join_probe_tile_kernel", "join_probe_lean2_kernel",
+              "agg_fast_kernel", "agg_fastreg_kernel", "agg_mid_kernel", "agg_mid2_kernel", "agg_priv_kernel",
+              "agg_wpriv_kernel", "agg_sink_kernel", "agg_rehash_kernel", "agg_fix_cnt_kernel", "agg_list_keys_kernel",
+              "agg_export_kernel", "agg_combine_kernel", "agg_export_packed_kernel", "agg_packed_header_kernel",
+              "agg_combine_packed_kernel", "fill_u64_kernel3"]:
         assert k in found, k
 
 
+def test_every_source_has_one_owner():
+    srcs = [s for v in MODULES.values() for s in v]
+    assert len(srcs) == len(set(srcs))
+    for s in srcs:
+        assert os.path.exists(os.path.join(CSRC, s)), s
+
+
 def test_every_fast_path_kernel_has_a_gpu_case():
-    cases, excluded, _ = gpu_module()
-    for src in SOURCES:
-        for k in sorted(kernels_in(os.path.join(CSRC, src))):
-            assert k in cases or k in excluded, \
-                f"{src}: kernel {k} has no case in KERNEL_CASES of test_gpu_kernel_paths.py and no exclusion"
-            if k in excluded:
-                assert isinstance(excluded[k], str) and excluded[k].strip(), f"{k}: an exclusion needs a reason"
+    for module, srcs in MODULES.items():
+        cases, excluded, _ = gpu_module(module)
+        for src in srcs:
+            for k in sorted(kernels_in(os.path.join(CSRC, src))):
+                assert k in cases or k in excluded, \
+                    f"{src}: kernel {k} has no case in KERNEL_CASES of {module} and no exclusion"
+                if k in excluded:
+                    assert isinstance(excluded[k], str) and excluded[k].strip(), f"{k}: an exclusion needs a reason"
 
 
 def test_kernel_cases_name_tests_that_check_the_kernel():
-    cases, excluded, funcs = gpu_module()
-    known = set().union(*(kernels_in(os.path.join(CSRC, s)) for s in SOURCES))
-    for k, tests in cases.items():
-        assert k in known, f"KERNEL_CASES lists {k}, which no longer exists"
-        assert k not in excluded, k
-        assert tests, k
-        for t in tests:
-            assert t.startswith("test_") and t in funcs, f"{k}: no test function {t}"
-            assert k in funcs[t], f"{t} does not name {k}: it cannot be asserting that the kernel ran"
+    for module, srcs in MODULES.items():
+        cases, excluded, funcs = gpu_module(module)
+        known = set().union(*(kernels_in(os.path.join(CSRC, s)) for s in srcs))
+        for k in excluded:
+            assert k in known, f"KERNEL_EXCLUDED of {module} lists {k}, which is not a kernel of its sources"
+        for k, tests in cases.items():
+            assert k in known, f"KERNEL_CASES of {module} lists {k}, which is not a kernel of its sources"
+            assert k not in excluded, k
+            assert tests, k
+            for t in tests:
+                assert t.startswith("test_") and t in funcs, f"{k}: no test function {t}"
+                assert k in funcs[t], f"{t} does not name {k}: it cannot be asserting that the kernel ran"
