@@ -73,6 +73,45 @@ __device__ __forceinline__ bool int_in_range(int type, int64_t v) {
 	}
 }
 
+// largest value of integer type t, as an unsigned 64-bit number
+__device__ __forceinline__ uint64_t int_max(int t) {
+	const int bits = b200_type_size(t) * 8;
+	if (b200_type_is_signed_int(t)) {
+		return (1ULL << (bits - 1)) - 1;
+	}
+	return bits == 64 ? ~0ULL : (1ULL << bits) - 1;
+}
+
+// Does the raw value s of an integer source (sign-extended when src_signed, zero-extended otherwise) lie in the range
+// of integer type t?  TryCastWithOverflowCheck (numeric_cast.hpp) for every signedness pair and both 64-bit types.
+__device__ __forceinline__ bool int_fits(int t, uint64_t s, bool src_signed) {
+	if (src_signed && (int64_t)s < 0) {
+		return b200_type_is_signed_int(t) && (int64_t)s >= -(int64_t)int_max(t) - 1;
+	}
+	return s <= int_max(t);
+}
+
+// the low bits of s that type t holds, sign- or zero-extended to 64 bits (the form eval_row keeps every raw value in)
+__device__ __forceinline__ uint64_t extend_raw(int t, uint64_t s) {
+	switch (t) {
+	case B200_INT8:
+		return (uint64_t)(int64_t)(int8_t)s;
+	case B200_INT16:
+		return (uint64_t)(int64_t)(int16_t)s;
+	case B200_INT32:
+		return (uint64_t)(int64_t)(int32_t)s;
+	case B200_BOOL:
+	case B200_UINT8:
+		return (uint8_t)s;
+	case B200_UINT16:
+		return (uint16_t)s;
+	case B200_UINT32:
+		return (uint32_t)s;
+	default:
+		return s;
+	}
+}
+
 __device__ __forceinline__ bool decimal_in_range(int type, int64_t v) {
 	switch (type) {
 	case B200_INT16:
@@ -217,31 +256,46 @@ __device__ __forceinline__ void eval_row(const ExprProg &p, uint64_t row, uint32
 				if (ovf && !isnull) {
 					*overflow = 1;
 				}
-				v = (uint64_t)r;
+				// unchecked results wrap to the width of their type (AddOperator etc.)
+				v = extend_raw(nd.type, (uint64_t)r);
 			}
 			break;
 		}
 		case B200_EXPR_CAST: {
-			// numeric widening cast between integer types / to double
+			// numeric cast with DuckDB's rules (TryCastWithOverflowCheck, numeric_cast.hpp): an integer must fit its
+			// target, a 64-bit integer rounds once to FLOAT, a finite DOUBLE must stay finite as FLOAT, and any integer
+			// becomes BOOL as `!= 0`.  FLOAT/DOUBLE -> integer is rejected by b200_filter_project.
 			isnull = nul[nd.left];
 			int st = p.nodes[nd.left].type;
 			uint64_t s = val[nd.left];
-			if (b200_type_is_float(nd.type)) {
-				double d;
-				if (b200_type_is_float(st)) {
-					d = raw_to_double(st, s);
+			bool ovf = false;
+			if (nd.type == B200_FLOAT) {
+				float f;
+				if (st == B200_DOUBLE) {
+					double d = __longlong_as_double((long long)s);
+					f = (float)d;
+					ovf = isfinite(d) && isinf(f);
+				} else if (st == B200_FLOAT) {
+					f = __uint_as_float((uint32_t)s);
 				} else if (b200_type_is_signed_int(st)) {
-					d = (double)(int64_t)s;
+					f = __ll2float_rn((long long)s);
 				} else {
-					d = (double)s;
+					f = __ull2float_rn(s);
 				}
-				v = nd.type == B200_FLOAT ? (uint64_t)__float_as_uint((float)d)
-				                          : (uint64_t)__double_as_longlong(d);
+				v = __float_as_uint(f);
+			} else if (nd.type == B200_DOUBLE) {
+				double d = b200_type_is_float(st)         ? raw_to_double(st, s)
+				           : b200_type_is_signed_int(st) ? __ll2double_rn((long long)s)
+				                                         : __ull2double_rn(s);
+				v = (uint64_t)__double_as_longlong(d);
+			} else if (nd.type == B200_BOOL) {
+				v = s != 0;
 			} else {
-				v = s; // raw values are already sign/zero extended to 64 bits
-				if (!isnull && !int_in_range(nd.type, (int64_t)s) && !(st == B200_UINT64 || nd.type == B200_UINT64)) {
-					*overflow = 1;
-				}
+				ovf = !int_fits(nd.type, s, b200_type_is_signed_int(st));
+				v = extend_raw(nd.type, s);
+			}
+			if (ovf && !isnull) {
+				*overflow = 1;
 			}
 			break;
 		}
@@ -572,6 +626,25 @@ extern "C" int b200_filter_project(b200_ctx *ctx, const b200_batch *in, const b2
 				               nodes[nd.right].type);
 				return B200_ERR_INVALID;
 			}
+		}
+		// DuckDB binds both operands of + - * to the result's type, and the interpreter reads them in that type.  The
+		// check mode (`col`) is 0 (wrap), 1 (range of the type) or 2 (DECIMAL bound: INT16, INT32 and INT64 only).
+		if (nd.op == B200_EXPR_ADD || nd.op == B200_EXPR_SUB || nd.op == B200_EXPR_MUL) {
+			if (nd.type == B200_BOOL || nodes[nd.left].type != nd.type || nodes[nd.right].type != nd.type) {
+				b200_set_error("b200_filter_project: node %d of type %d has operands of type %d and %d", i, nd.type,
+				               nodes[nd.left].type, nodes[nd.right].type);
+				return B200_ERR_INVALID;
+			}
+			bool decimal = nd.type == B200_INT16 || nd.type == B200_INT32 || nd.type == B200_INT64;
+			if (!b200_type_is_float(nd.type) && (nd.col < 0 || nd.col > 2 || (nd.col == 2 && !decimal))) {
+				b200_set_error("b200_filter_project: node %d has check mode %d for type %d", i, nd.col, nd.type);
+				return B200_ERR_INVALID;
+			}
+		}
+		// FLOAT/DOUBLE -> integer casts (rounding, range of the rounded value) are not implemented
+		if (nd.op == B200_EXPR_CAST && b200_type_is_float(nodes[nd.left].type) && !b200_type_is_float(nd.type)) {
+			b200_set_error("b200_filter_project: node %d casts type %d to type %d", i, nodes[nd.left].type, nd.type);
+			return B200_ERR_INVALID;
 		}
 		if (nd.op == B200_EXPR_CONST && !nd.is_null && b200_type_is_integer(nd.type) && b200_type_size(nd.type) < 8) {
 			const int bits = b200_type_size(nd.type) * 8;

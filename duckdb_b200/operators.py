@@ -182,9 +182,11 @@ class Batch:
         return [self.download(i) for i in range(self.ncols)]
 
     def free(self):
-        if self.handle:
+        # b200_batch_free returns the columns to the batch's context: once that context is closed (a batch kept alive
+        # by a reference cycle can outlive it) there is nothing left to free them to, and the call would read freed memory
+        if self.handle and self.ctx.handle:
             lib().b200_batch_free(self.handle)
-            self.handle = C.c_void_p()
+        self.handle = C.c_void_p()
 
     def __del__(self):
         try:

@@ -164,13 +164,11 @@ typedef enum b200_expr_op {
 	B200_EXPR_NOT_DISTINCT = 40,
 	B200_EXPR_AND = 50,
 	B200_EXPR_OR = 51,
-	/* arithmetic on integers (DECIMAL is physical int): overflow is an error,
-	 * like DecimalAddOverflowCheck / MultiplyOperatorOverflowCheck
-	 * (src/function/scalar/operator/arithmetic.cpp:975-1008). */
+	/* arithmetic (DECIMAL is physical int) and numeric casts: rules below b200_expr_node */
 	B200_EXPR_ADD = 1001,
 	B200_EXPR_SUB = 1002,
 	B200_EXPR_MUL = 1003,
-	B200_EXPR_CAST = 1004     /* numeric widening cast of `left` to `type`        */
+	B200_EXPR_CAST = 1004     /* numeric cast of `left` to `type`                  */
 } b200_expr_op;
 
 /* limits of one b200_filter_project call (programs beyond them return B200_ERR_INVALID) */
@@ -192,7 +190,25 @@ typedef struct b200_expr_node {
 	} value;          /* CONST payload; an integer constant must be representable in `type` */
 } b200_expr_node;
 /* The two operands of a comparison (EQ .. GE, DISTINCT, NOT_DISTINCT) must have the same type;
- * b200_filter_project returns B200_ERR_INVALID otherwise. */
+ * b200_filter_project returns B200_ERR_INVALID otherwise.
+ *
+ * ADD, SUB, MUL: both operands have the node's type (B200_ERR_INVALID otherwise; BOOL is not allowed).  On
+ * integers `col` selects the overflow check, made only for rows whose operands are not NULL and only where the
+ * expression is evaluated (projections: surviving rows only); a failed check makes the call return
+ * B200_ERR_OVERFLOW:
+ *   0  none: the result wraps to the width of its type (AddOperator, add.cpp)
+ *   1  the range of the type (TryAddOperator / TrySubtractOperator / TryMultiplyOperator)
+ *   2  the DECIMAL bound of the type: 9999 (INT16), 999999999 (INT32), 10^18 - 1 (INT64); other types
+ *      return B200_ERR_INVALID (DecimalAddOverflowCheck etc., arithmetic.cpp:975-1008)
+ * FLOAT / DOUBLE arithmetic is IEEE in the node's type, rounded once.
+ *
+ * CAST, like TryCastWithOverflowCheck (numeric_cast.hpp:27-72,187-197):
+ *   integer -> integer  the value must lie in the target's range (any signedness, any width), else overflow
+ *   integer -> BOOL     value != 0
+ *   integer -> FLOAT / DOUBLE  rounded once to nearest even
+ *   DOUBLE -> FLOAT     rounded to nearest; a finite value that becomes infinite is an overflow (NaN and
+ *                       infinities pass through)
+ *   FLOAT / DOUBLE -> integer  not supported: B200_ERR_INVALID */
 
 /* One pass of PhysicalFilter (+ the PhysicalProjection above it):
  *   rows for which node `filter_root` is TRUE (not NULL, not false) survive

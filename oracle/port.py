@@ -182,10 +182,36 @@ def eval_expr(node, cols, n):
         wrapped = np.array([int(x) & mask for x in r], dtype=np.uint64).astype(np.dtype(f"u{dt.itemsize}"))
         return wrapped.view(dt) if dt.kind == "i" else wrapped, valid
     if op == "cast":
-        dt = np.dtype(node[1])
         a, av = eval_expr(node[2], cols, n)
-        return a.astype(dt), av
+        return cast(a, av, np.dtype(node[1])), av
     raise ValueError(op)
+
+
+def cast(a, valid, dt):
+    """CAST of the values a (valid rows only can fail) to dtype dt with DuckDB's numeric rules
+    (TryCastWithOverflowCheck, numeric_cast.hpp:27-72,187-197): an integer outside the target's range and a finite
+    DOUBLE that becomes an infinite FLOAT raise OverflowError_; integers round once to FLOAT / DOUBLE; an integer
+    becomes BOOLEAN as `!= 0`.  FLOAT / DOUBLE -> integer is not supported (ValueError)."""
+    a = np.asarray(a)
+    if a.dtype.kind == "f":
+        if dt.kind != "f":
+            raise ValueError(f"cast {a.dtype} -> {dt} is not supported")
+        with np.errstate(over="ignore"):
+            r = a.astype(dt)
+        if (np.isfinite(a) & np.isinf(r) & valid).any():
+            raise OverflowError_("overflow")
+        return r
+    if dt == np.bool_:
+        return a != 0
+    if dt.kind == "f":
+        return a.astype(dt)  # one rounding: numpy converts 64-bit integers to float32 directly
+    lo, hi = _INT_RANGE[dt]
+    ints = [int(x) for x in a]
+    if any(ok and not lo <= x <= hi for x, ok in zip(ints, valid)):
+        raise OverflowError_("overflow")
+    mask = (1 << (dt.itemsize * 8)) - 1
+    wrapped = np.array([x & mask for x in ints], dtype=np.uint64).astype(np.dtype(f"u{dt.itemsize}"))
+    return wrapped.view(dt)
 
 
 def filter_select(pred, cols, n):

@@ -14,6 +14,8 @@ Outputs (committed):
   reference_results.json  the reference's answers for the tests that compare with it (see reference_results())
   reference_avg.npz       the reference's avg(d) of every group of test_gpu_parity's group-by, as the exact bit
                           difference from numpy's bincount mean (mostly 0 to a few units in the last place: the file stays small)
+  expr_cases.json  the reference's result (or "error") of numeric CASTs and checked integer + - * at the edges
+                   (expr_edge_cases())
 """
 import json
 import os
@@ -380,10 +382,107 @@ def reference_results(con):
         fh.write("\n")
 
 
+INT_NAMES = ["int8", "uint8", "int16", "uint16", "int32", "uint32", "int64", "uint64"]
+
+
+def _int_edges(name):
+    """the limits of an integer type, +-1 around them and around 0, and the square-root and halving edges of MUL/ADD"""
+    info = np.iinfo(name)
+    lo, hi = int(info.min), int(info.max)
+    r = int(np.sqrt(float(hi)))
+    while (r + 1) * (r + 1) <= hi:
+        r += 1
+    while r * r > hi:
+        r -= 1
+    vals = {lo, lo + 1, -1, 0, 1, 2, hi // 2, hi // 2 + 1, r, r + 1, -r - 1, hi - 1, hi}
+    return sorted(v for v in vals if lo <= v <= hi)
+
+
+# integers whose conversion to FLOAT rounds differently when it goes through DOUBLE first, and integers near 2^53,
+# 2^63 and 2^64 (UBIGINT values just below 2^64 round up to 2^64 as FLOAT)
+ROUNDING_INTS = [2 ** 60 + 2 ** 36 + 1, 2 ** 60 + 2 ** 36, 2 ** 60 + 2 ** 36 - 1, 2 ** 53 + 1, 2 ** 53 - 1, 2 ** 24 + 1,
+                 2 ** 62 + 2 ** 38 + 1, 2 ** 63 - 2 ** 39, 2 ** 63 - 2 ** 39 + 1, 2 ** 63, 2 ** 63 + 2 ** 39 + 1,
+                 2 ** 64 - 2 ** 40 + 1, 2 ** 64 - 2 ** 39 - 1, 2 ** 64 - 2 ** 39, 2 ** 64 - 2 ** 39 + 1, 2 ** 64 - 2,
+                 -(2 ** 60 + 2 ** 36 + 1), -(2 ** 53 + 1), -(2 ** 63 - 2 ** 39 + 1)]
+FLT_MAX = float(np.finfo(np.float32).max)
+# doubles at the FLOAT limits: FLT_MAX and the half-way point above it (which rounds to infinity), the smallest
+# subnormals, a value that underflows to zero, and the non-finite values that pass through
+DOUBLE_EDGES = [0.0, -0.0, 0.1, 1.5, -2.75, FLT_MAX, -FLT_MAX, 2.0 ** 128 - 2.0 ** 103, np.nextafter(2.0 ** 128 - 2.0 ** 103, 0),
+                -(2.0 ** 128 - 2.0 ** 103), 2.0 ** 128, 1e300, -1e300, 2.0 ** -149, 2.0 ** -150, 3 * 2.0 ** -151, 1e-50,
+                float("inf"), float("-inf"), float("nan"), 16777217.0, 1.0 + 2.0 ** -24 + 2.0 ** -52]
+FLOAT_EDGES = [0.0, -0.0, 1.5, FLT_MAX, -FLT_MAX, 2.0 ** -149, float(np.float32(0.1)), float("inf"), float("-inf"),
+               float("nan")]
+
+
+def _enc(x, name):
+    """a value of type `name` as JSON: integers exact, floats as float.hex (which keeps inf and nan)"""
+    return float(x).hex() if name in ("float32", "float64") else (bool(x) if name == "bool" else int(x))
+
+
+def _sql_lit(x, name):
+    if name in ("float32", "float64"):
+        return repr(float(x))
+    return str(int(x))
+
+
+def expr_edge_cases():
+    """-> [{op, type, src?, args}]: every CAST pair among the integer types, integer -> FLOAT / DOUBLE / BOOLEAN,
+    FLOAT -> DOUBLE and DOUBLE -> FLOAT, and ADD / SUB / MUL in every integer type, with operands at the edges"""
+    cases = []
+    for src in INT_NAMES:
+        info = np.iinfo(src)
+        for dst in INT_NAMES + ["bool", "float32", "float64"]:
+            vals = set(_int_edges(src))
+            if dst in INT_NAMES:
+                d = np.iinfo(dst)
+                vals |= {int(d.min) - 1, int(d.min), int(d.max), int(d.max) + 1}
+            elif dst != "bool" and src in ("int64", "uint64"):
+                vals |= set(ROUNDING_INTS)
+            for x in sorted(v for v in vals if info.min <= v <= info.max):
+                cases.append({"op": "cast", "src": src, "type": dst, "args": [x]})
+    for x in FLOAT_EDGES:
+        cases.append({"op": "cast", "src": "float32", "type": "float64", "args": [x]})
+    for x in DOUBLE_EDGES:
+        cases.append({"op": "cast", "src": "float64", "type": "float32", "args": [float(x)]})
+    for t in INT_NAMES:
+        edges = _int_edges(t)
+        for op in ("add", "sub", "mul"):
+            for a in edges:
+                for b in edges:
+                    cases.append({"op": op, "type": t, "args": [a, b]})
+    return cases
+
+
+def expr_cases(con):
+    """expr_cases.json: DuckDB's result of every case of expr_edge_cases(), each in its own query, or "error" when the
+    query fails with a conversion or overflow error"""
+    sql_type = {np.dtype(k).name: v for k, v in R._SQL_OF_NP.items()}
+    sym = {"add": "+", "sub": "-", "mul": "*"}
+    out = []
+    for case in expr_edge_cases():
+        t = case["type"]
+        if case["op"] == "cast":
+            sql = f"SELECT CAST(CAST('{_sql_lit(case['args'][0], case['src'])}' AS {sql_type[case['src']]}) AS {sql_type[t]})"
+        else:
+            a, b = (f"CAST('{_sql_lit(x, t)}' AS {sql_type[t]})" for x in case["args"])
+            sql = f"SELECT {a} {sym[case['op']]} {b}"
+        try:
+            col = con.execute(sql)[0]
+            assert col.values.dtype == np.dtype(t), (sql, col.values.dtype)
+            result = _enc(col.values[0], t)
+        except RuntimeError as e:
+            assert any(k in str(e) for k in ("Conversion Error", "Out of Range", "Overflow")), (sql, str(e))
+            result = "error"
+        out.append(dict(case, args=[_enc(x, case.get("src", t)) for x in case["args"]], result=result))
+    with open(os.path.join(OUT, "expr_cases.json"), "w") as fh:
+        json.dump(out, fh, separators=(",", ":"))
+        fh.write("\n")
+
+
 def main():
     """With arguments: only the named fixtures (e.g. `reference_results`), so that the others are not rewritten."""
     con = R.Connection(threads=4)
-    for fn in sys.argv[1:] or ["hash_kat", "filter_cases", "join_cases", "tpch", "reference_results"]:
+    for fn in sys.argv[1:] or ["hash_kat", "filter_cases", "join_cases", "tpch", "reference_results", "expr_cases"]:
         globals()[fn](con)
     con.close()
     for f in sorted(os.listdir(OUT)):

@@ -8,6 +8,13 @@ import json
 import os
 import re
 import tempfile
+import time
+
+# The profiler keeps only the GPU activities whose timestamps fall inside the window it measures on the host clock, and
+# the two clocks disagree by a few milliseconds (a kernel's reported start lay between 2.9 ms before and 3.5 ms after
+# its host-side launch on an H100).  A window shorter than that offset, such as one around a single small kernel, can
+# lose every kernel.  Idle margins on both sides of the block keep what it launches inside the window.
+WINDOW_MARGIN_S = 0.02
 
 
 def _strip(name):
@@ -34,8 +41,10 @@ def kernel_trace():
     names = []
     torch.cuda.synchronize()
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        time.sleep(WINDOW_MARGIN_S)
         yield names
         torch.cuda.synchronize()
+        time.sleep(WINDOW_MARGIN_S)
     with tempfile.TemporaryDirectory() as d:
         path = os.path.join(d, "trace.json")
         prof.export_chrome_trace(path)
@@ -71,9 +80,9 @@ def assert_not_ran(names, *kernels):
 
 
 def traced(fn):
-    """-> (fn(), kernel names).  A window in which the profiler delivered no kernel at all (CUPTI occasionally drops a
-    whole window's activity records) is not evidence about the dispatcher: fn, which must be repeatable, runs once more
-    in a fresh window, and a second empty window is an error."""
+    """-> (fn(), kernel names).  A window in which the profiler delivered no kernel at all is not evidence about the
+    dispatcher: fn, which must be repeatable, runs once more in a fresh window, and a second empty window is an
+    error."""
     for attempt in range(2):
         with kernel_trace() as names:
             result = fn()

@@ -1,4 +1,4 @@
-"""Every __global__ kernel of the fast-path and aggregate sources is claimed by a case of the GPU module that owns the
+"""Every __global__ kernel of the fast-path, aggregate and generic filter sources is claimed by a case of the GPU module that owns the
 source (which asserts, through the kernel trace, that it ran) or excluded there with a reason: a new kernel variant
 fails this test until a GPU case covers it."""
 import ast
@@ -11,6 +11,7 @@ CSRC = os.path.join(ROOT, "duckdb_b200", "csrc")
 MODULES = {
     "test_gpu_kernel_paths.py": ["filter_tile.cu", "agg_hc.cu", "join_tile.cu"],
     "test_gpu_agg_kernel_paths.py": ["agg_tile.cu", "agg_priv.cu", "agg.cu"],
+    "test_gpu_filter_interpreter.py": ["filter.cu"],
 }
 
 _GLOBAL = re.compile(r"__global__\s+void\s+(?:__launch_bounds__\s*\([^()]*\)\s*)?(\w+)\s*\(")
@@ -43,7 +44,8 @@ def test_parser_finds_the_known_kernels():
               "agg_fast_kernel", "agg_fastreg_kernel", "agg_mid_kernel", "agg_mid2_kernel", "agg_priv_kernel",
               "agg_wpriv_kernel", "agg_sink_kernel", "agg_rehash_kernel", "agg_fix_cnt_kernel", "agg_list_keys_kernel",
               "agg_export_kernel", "agg_combine_kernel", "agg_export_packed_kernel", "agg_packed_header_kernel",
-              "agg_combine_packed_kernel", "fill_u64_kernel3"]:
+              "agg_combine_packed_kernel", "fill_u64_kernel3", "filter_mask_kernel", "compact_kernel",
+              "tile_scan_local_kernel", "tile_scan_chunks_kernel", "tile_scan_add_kernel", "fill_u64_kernel2"]:
         assert k in found, k
 
 

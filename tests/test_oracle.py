@@ -1,9 +1,12 @@
 """The CPU oracle (oracle/port.py) pinned against the reference's own known-answer vectors and the golden
 fixtures generated from the unmodified reference."""
+import json
+import os
+
 import numpy as np
 import pytest
 
-from conftest import assert_matches, digest_array, golden
+from conftest import GOLDEN, assert_matches, digest_array, golden
 from oracle import port as P
 
 
@@ -72,6 +75,74 @@ def test_projection_golden():
     v, valid = P.eval_expr(("add", np.int32, ("col", 0), ("col", 1), 1), cols, n)
     np.testing.assert_array_equal(valid[sel], g["proj_add_valid"])
     np.testing.assert_array_equal(v[sel][valid[sel]], g["proj_add"][g["proj_add_valid"]])
+
+
+INT_NAMES = ["int8", "uint8", "int16", "uint16", "int32", "uint32", "int64", "uint64"]
+
+
+def expr_cases():
+    """The reference's result ("error" when it raised) of numeric CASTs and checked + - * with operands at the edges
+    (tests/golden/make_golden.py expr_cases): [{op, type, src (CAST only), args, result}], floats as float.hex."""
+    with open(os.path.join(GOLDEN, "expr_cases.json")) as f:
+        return json.load(f)
+
+
+def decode(x, name):
+    """a JSON value of expr_cases.json -> a Python value of dtype `name`"""
+    if name in ("float32", "float64"):
+        return float(np.dtype(name).type(float.fromhex(x)))
+    return bool(x) if name == "bool" else int(x)
+
+
+def encode(x, name):
+    return float(x).hex() if name in ("float32", "float64") else (bool(x) if name == "bool" else int(x))
+
+
+def expr_case_tree(case, mode=1):
+    """the case as an oracle expression over constants"""
+    if case["op"] == "cast":
+        return ("cast", np.dtype(case["type"]), ("const", decode(case["args"][0], case["src"]), np.dtype(case["src"])))
+    dt = np.dtype(case["type"])
+    a, b = (("const", decode(x, case["type"]), dt) for x in case["args"])
+    return (case["op"], dt, a, b, mode)
+
+
+def test_expr_cases_golden():
+    """the port's CAST and checked integer arithmetic equal the reference's answer in every edge case: the value,
+    bit for bit, or an overflow error"""
+    cases = expr_cases()
+    pairs = {(c["src"], c["type"]) for c in cases if c["op"] == "cast"}
+    assert pairs == {(s, d) for s in INT_NAMES for d in INT_NAMES + ["bool", "float32", "float64"]} | \
+        {("float32", "float64"), ("float64", "float32")}
+    assert {(c["op"], c["type"]) for c in cases if c["op"] != "cast"} == \
+        {(op, t) for op in ("add", "sub", "mul") for t in INT_NAMES}
+    assert sum(c["result"] == "error" for c in cases) > 1000
+    for case in cases:
+        try:
+            v, valid = P.eval_expr(expr_case_tree(case), [], 1)
+            got = encode(v[0], case["type"])
+            assert valid[0]
+        except P.OverflowError_:
+            got = "error"
+        assert got == case["result"], case
+    # the port's unchecked arithmetic wraps: the exact result modulo 2^width, read in the type
+    for case in cases:
+        if case["op"] != "cast":
+            v, _ = P.eval_expr(expr_case_tree(case, mode=0), [], 1)
+            a, b = (int(x) for x in case["args"])
+            exact = {"add": a + b, "sub": a - b, "mul": a * b}[case["op"]]
+            bits = np.dtype(case["type"]).itemsize * 8
+            lo = -(1 << (bits - 1)) if case["type"].startswith("int") else 0
+            assert int(v[0]) == (exact - lo) % (1 << bits) + lo, case
+
+
+def test_port_cast_rejects_float_to_integer():
+    with pytest.raises(ValueError):
+        P.eval_expr(("cast", np.dtype(np.int64), ("const", 1.0, np.float32)), [], 1)
+    # NULL rows never overflow
+    v, valid = P.eval_expr(("cast", np.dtype(np.uint8), ("col", 0)),
+                           [(np.array([300, 7], dtype=np.int64), np.array([False, True]))], 2)
+    assert int(v[1]) == 7 and valid.tolist() == [False, True]
 
 
 def test_config1_golden():
