@@ -667,6 +667,13 @@ int b200_radix_partition(b200_ctx *ctx, const b200_batch *in, const int *key_col
 		b200_set_error("b200_radix_partition: at most 2^32-1 rows per batch");
 		return B200_ERR_INVALID;
 	}
+	// both paths move values as at most 8 bytes (the fast path's width switch, store_raw / col_load_raw)
+	for (size_t ci = 0; ci < in->cols.size(); ci++) {
+		if (in->cols[ci].type == B200_INT128) {
+			b200_set_error("b200_radix_partition: INT128 columns are not supported (column %d)", (int)ci);
+			return B200_ERR_INVALID;
+		}
+	}
 	KeyCols keys;
 	B200_TRY(b200_fill_keycols(in, key_cols, nkeys, &keys, "b200_radix_partition"));
 	CUDA_TRY(cudaSetDevice(ctx->device));
@@ -812,6 +819,11 @@ static int part_fast_eligible(const b200_batch *in, int bits, PartCols *pc, size
 		const DCol &c = in->cols[ci];
 		if (c.vtype != B200_FLAT_VECTOR || c.validity) {
 			b200_set_error("%s: column %d must be a flat vector without NULLs", who, ci);
+			return B200_ERR_INVALID;
+		}
+		if (c.type == B200_INT128) {
+			// the move kernels copy values of 1, 2, 4 or 8 bytes
+			b200_set_error("%s: INT128 columns are not supported (column %d)", who, ci);
 			return B200_ERR_INVALID;
 		}
 		pc->in[ci] = c.data;

@@ -658,6 +658,11 @@ int b200_join_probe(b200_join *j, const b200_batch *probe, const int *key_cols, 
 			b200_set_error("b200_join_probe: lhs column index %d out of range", lhs_cols[i]);
 			return B200_ERR_INVALID;
 		}
+		// the probe kernels copy lhs values as at most 8 bytes (emit_row / the tile kernel's copy_value)
+		if (probe->cols[lhs_cols[i]].type == B200_INT128) {
+			b200_set_error("b200_join_probe: INT128 lhs columns are not supported (lhs column %d)", i);
+			return B200_ERR_INVALID;
+		}
 	}
 	uint64_t n = probe->nrows;
 	if (n > 0xffffffffULL) {

@@ -310,7 +310,9 @@ typedef struct b200_join b200_join; /* = HashJoinGlobalSinkState + JoinHashTable
 
 /* Replaces PhysicalHashJoin's sink state / JoinHashTable construction
  * (physical_hash_join.cpp:764-834; join_hashtable.cpp).  Conditions are
- * equality on nkeys key columns (NULL keys never match: join_hashtable.cpp:714-742). */
+ * equality on nkeys key columns (NULL keys never match: join_hashtable.cpp:714-742).
+ * Key and payload columns: any b200_type except B200_INT128 (B200_ERR_INVALID);
+ * 1..8 key columns, 0..12 payload columns. */
 B200_API int b200_join_create(b200_ctx *ctx, int join_type, const int32_t *key_types, int nkeys,
                               const int32_t *payload_types, int npayload, b200_join **out);
 /* Append build-side rows.  Replaces PhysicalHashJoin::Sink -> JoinHashTable::Build
@@ -334,6 +336,9 @@ B200_API int b200_join_build_rows(b200_join *join, uint64_t *out_rows);
  *       NULL) after the lhs columns.
  * out_capacity bounds the result rows (B200_ERR_CAPACITY if exceeded; pass 0
  * to let the library size it exactly with a counting pass).
+ * Probe key columns have the types the join was created with; lhs columns
+ * (at most 12) may be of any b200_type except B200_INT128 (B200_ERR_INVALID),
+ * and flat, constant or dictionary vectors, like the keys.
  * Result order is unspecified (SURVEY.md 3.3).
  * Replaces PhysicalHashJoin::ExecuteInternal -> JoinHashTable::Probe /
  * ScanStructure::Next* / GatherRHS (physical_hash_join.cpp:2140-2209;
@@ -350,6 +355,8 @@ B200_API void b200_join_destroy(b200_join *join);
  * partition id is the GPU rank of an 8-GPU box.  out has the same columns as
  * `in` (flat), rows grouped by partition; counts_host[p] = rows of partition p
  * (2^bits entries).  Row order inside a partition is unspecified.
+ * bits 0..12; 1..8 key columns; columns of any b200_type except B200_INT128
+ * (B200_ERR_INVALID), flat, constant or dictionary, with or without NULLs.
  * Replaces PartitionedTupleData::AppendUnified (partitioned_tuple_data.cpp:62-96). */
 B200_API int b200_radix_partition(b200_ctx *ctx, const b200_batch *in, const int *key_cols, int nkeys, int bits,
                                   b200_batch **out, uint64_t *counts_host);
@@ -369,7 +376,9 @@ B200_API int b200_radix_partition(b200_ctx *ctx, const b200_batch *in, const int
  *      stored to dst_cols[p * ncols + c] at row dst_row_offsets[p] + (rank of the
  *      row among this source's rows of partition p; order unspecified).  The
  *      destination pointers may be local or peer-mapped device memory.
- * Restrictions: bits <= 4, flat columns without NULLs (the shuffle path). */
+ * Restrictions: bits <= 4, 1..16 flat columns without NULLs of at most 48 bytes
+ * per row, no B200_INT128 column (the shuffle path; B200_ERR_INVALID otherwise).
+ * The _dev forms below have the same restrictions. */
 B200_API int b200_partition_count(b200_ctx *ctx, const b200_batch *in, const int *key_cols, int nkeys, int bits,
                                   uint64_t *counts_host);
 B200_API int b200_partition_scatter(b200_ctx *ctx, const b200_batch *in, const int *key_cols, int nkeys, int bits,

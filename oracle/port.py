@@ -31,6 +31,31 @@ def murmur64(x):
     return x
 
 
+_MASK64 = (1 << 64) - 1
+_M_INV = pow(0xD6E8FEB86659FD93, -1, 1 << 64)
+
+
+def murmur64_inverse(h):
+    """the 64-bit word x with murmur64(x) == h (Python ints).  Each step of murmur64 is a bijection: the xor-shift by 32
+    is its own inverse and the odd multiplier has an inverse modulo 2^64."""
+    x = int(h) & _MASK64
+    x ^= x >> 32
+    x = (x * _M_INV) & _MASK64
+    x ^= x >> 32
+    x = (x * _M_INV) & _MASK64
+    x ^= x >> 32
+    return x
+
+
+def combine_hash_preimage(prefix_hash, target):
+    """the BIGINT / UBIGINT key bits b (Python int) that give combine_hash(prefix_hash, murmur64(b)) == target: lets a test
+    give two different composite keys the same 64-bit hash, or a composite key any hash it wants"""
+    a = int(prefix_hash) & _MASK64
+    a ^= a >> 32
+    a = (a * int(_M)) & _MASK64
+    return murmur64_inverse((int(target) & _MASK64) ^ a)
+
+
 def hash_values(values):
     """duckdb::Hash<T> (hash.hpp:47-54, hash.cpp:33-57): ints < 64 bit hash their uint32 cast;
     floats: -0.0 -> +0.0 and NaN -> canonical quiet NaN, then the raw bits."""

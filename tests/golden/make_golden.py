@@ -16,6 +16,8 @@ Outputs (committed):
                           difference from numpy's bincount mean (mostly 0 to a few units in the last place: the file stays small)
   expr_cases.json  the reference's result (or "error") of numeric CASTs and checked integer + - * at the edges
                    (expr_edge_cases())
+  join_edge_cases.npz  composite-key joins with NULLs, +-0.0, NaN and type limits, and single-key MARK joins against
+                   all-NULL, empty and NULL-holding build sides
 """
 import json
 import os
@@ -202,6 +204,60 @@ def join_cases(con):
     out.update(b2=b2, p2=p2)
     out["inner2_id"], out["inner2_p"] = r[0].values, r[1].values
     np.savez_compressed(os.path.join(OUT, "join_cases.npz"), **out)
+
+
+def join_edge_keys(rng, n):
+    """composite join keys (BIGINT, DOUBLE, SMALLINT) drawn from small pools of edge values (type limits, +-0.0, NaN,
+    infinities) so that duplicates and cross-side matches are common, with NULLs in every key position"""
+    a = rng.choice(np.array([-2 ** 63, 2 ** 63 - 1, 0, 1, -1, 2 ** 62], dtype=np.int64), size=n)
+    d = rng.choice(np.array([0.0, -0.0, np.nan, 1.5, -np.inf, np.inf, np.finfo(np.float64).max], dtype=np.float64),
+                   size=n)
+    s = rng.choice(np.array([-32768, 32767, 0, -1], dtype=np.int16), size=n)
+    valid = [rng.random(n) > 0.08 for _ in range(3)]
+    return (a, valid[0]), (d, valid[1]), (s, valid[2])
+
+
+def join_edge_cases(con):
+    """join_edge_cases.npz: the semantics the oracle is pinned on beyond join_cases.npz.
+    Composite keys (BIGINT, DOUBLE, SMALLINT) with NULLs in every position, +-0.0, NaN and the type limits: INNER,
+    LEFT, SEMI and ANTI results as (probe id, build id) pairs.  Single-key MARK (`k IN (SELECT k FROM b)`) against a
+    build side of only NULL keys, an empty one and one with a NULL key among others."""
+    rng = np.random.default_rng(2024)   # its own generator: the file regenerates identically when run by name
+    out = {}
+    nb, npb = 300, 400
+    bcols, pcols = join_edge_keys(rng, nb), join_edge_keys(rng, npb)
+    con.load_table("cb", {"a": bcols[0], "d": bcols[1], "s": bcols[2], "id": np.arange(nb, dtype=np.int32)})
+    con.load_table("cp", {"a": pcols[0], "d": pcols[1], "s": pcols[2], "id": np.arange(npb, dtype=np.int32)})
+    for side, cols in (("b", bcols), ("p", pcols)):
+        for name, (v, valid) in zip("ads", cols):
+            out[f"{side}_{name}"], out[f"{side}_{name}_valid"] = v, valid
+    con.execute("SET disabled_optimizers='join_filter_pushdown'")
+    on = "cp.a = cb.a AND cp.d = cb.d AND cp.s = cb.s"
+    r = con.fetchall(f"SELECT cp.id, cb.id FROM cp JOIN cb ON {on} ORDER BY 1, 2")
+    out["inner"] = np.array(r, dtype=np.int32).reshape(-1, 2)
+    r = con.fetchall(f"SELECT cp.id, cb.id FROM cp LEFT JOIN cb ON {on}")
+    out["left"] = np.array(sorted((p, -1 if b is None else b) for p, b in r), dtype=np.int32).reshape(-1, 2)
+    out["semi"] = con.execute(f"SELECT id FROM cp SEMI JOIN cb ON {on} ORDER BY 1")[0].values.astype(np.int32)
+    out["anti"] = con.execute(f"SELECT id FROM cp ANTI JOIN cb ON {on} ORDER BY 1")[0].values.astype(np.int32)
+    # single-key MARK
+    npm = 50
+    mk = rng.integers(0, 8, size=npm).astype(np.int64)
+    mkv = rng.random(npm) > 0.2
+    con.load_table("mp", {"k": (mk, mkv), "id": np.arange(npm, dtype=np.int32)})
+    out["mp_k"], out["mp_k_valid"] = mk, mkv
+    builds = {
+        "nulls": (np.arange(5, dtype=np.int64), np.zeros(5, dtype=bool)),
+        "empty": (np.zeros(0, dtype=np.int64), np.zeros(0, dtype=bool)),
+        "mixed": (np.array([1, 3, 5, 0, 7], dtype=np.int64), np.array([True, True, True, False, True])),
+    }
+    for name, (k, kv) in builds.items():
+        con.load_table(f"mb_{name}", {"k": (k, kv)})
+        r = con.execute(f"SELECT id, k IN (SELECT k FROM mb_{name}) FROM mp ORDER BY id")
+        out[f"mb_{name}_k"], out[f"mb_{name}_k_valid"] = k, kv
+        m, mv = col_arrays(r[1])
+        out[f"mark_{name}"], out[f"mark_{name}_valid"] = np.where(mv, m, False).astype(bool), mv   # NULL rows: False
+    con.execute("RESET disabled_optimizers")
+    np.savez_compressed(os.path.join(OUT, "join_edge_cases.npz"), **out)
 
 
 def _enum_values(path, enum_name):
@@ -482,7 +538,8 @@ def expr_cases(con):
 def main():
     """With arguments: only the named fixtures (e.g. `reference_results`), so that the others are not rewritten."""
     con = R.Connection(threads=4)
-    for fn in sys.argv[1:] or ["hash_kat", "filter_cases", "join_cases", "tpch", "reference_results", "expr_cases"]:
+    for fn in sys.argv[1:] or ["hash_kat", "filter_cases", "join_cases", "tpch", "reference_results", "expr_cases",
+                                     "join_edge_cases"]:
         globals()[fn](con)
     con.close()
     for f in sorted(os.listdir(OUT)):

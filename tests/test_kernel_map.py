@@ -1,4 +1,4 @@
-"""Every __global__ kernel of the fast-path, aggregate and generic filter sources is claimed by a case of the GPU module that owns the
+"""Every __global__ kernel of the fast-path, aggregate, generic filter, join and partition sources is claimed by a case of the GPU module that owns the
 source (which asserts, through the kernel trace, that it ran) or excluded there with a reason: a new kernel variant
 fails this test until a GPU case covers it."""
 import ast
@@ -12,6 +12,7 @@ MODULES = {
     "test_gpu_kernel_paths.py": ["filter_tile.cu", "agg_hc.cu", "join_tile.cu"],
     "test_gpu_agg_kernel_paths.py": ["agg_tile.cu", "agg_priv.cu", "agg.cu"],
     "test_gpu_filter_interpreter.py": ["filter.cu"],
+    "test_gpu_join_kernels.py": ["join.cu", "hash.cu"],
 }
 
 _GLOBAL = re.compile(r"__global__\s+void\s+(?:__launch_bounds__\s*\([^()]*\)\s*)?(\w+)\s*\(")
@@ -45,7 +46,12 @@ def test_parser_finds_the_known_kernels():
               "agg_wpriv_kernel", "agg_sink_kernel", "agg_rehash_kernel", "agg_fix_cnt_kernel", "agg_list_keys_kernel",
               "agg_export_kernel", "agg_combine_kernel", "agg_export_packed_kernel", "agg_packed_header_kernel",
               "agg_combine_packed_kernel", "fill_u64_kernel3", "filter_mask_kernel", "compact_kernel",
-              "tile_scan_local_kernel", "tile_scan_chunks_kernel", "tile_scan_add_kernel", "fill_u64_kernel2"]:
+              "tile_scan_local_kernel", "tile_scan_chunks_kernel", "tile_scan_add_kernel", "fill_u64_kernel2",
+              "join_append_kernel", "join_append_col_kernel", "join_init_slots_kernel", "join_insert_kernel",
+              "join_minmax_kernel", "join_dense_build_kernel", "join_inline_kernel", "join_probe_kernel",
+              "fill_u64_kernel4", "hash_kernel", "part_hist_kernel", "part_scatter_index_kernel",
+              "part_scatter_col_kernel", "fill_u64_kernel", "exclusive_scan_small_kernel", "part_count_kernel",
+              "part_move_staged_kernel", "part_move_reg_kernel"]:
         assert k in found, k
 
 

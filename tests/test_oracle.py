@@ -211,6 +211,56 @@ def test_join_golden():
     assert got == sorted(zip(g["inner2_id"].tolist(), g["inner2_p"].tolist()))
 
 
+def test_join_edge_cases_golden():
+    """composite keys with NULLs in every position, +-0.0, NaN and type limits (INNER / LEFT / SEMI / ANTI), and
+    single-key MARK against all-NULL, empty and NULL-holding build sides: the port against the reference"""
+    g = golden("join_edge_cases.npz")
+    bkeys = [(g[f"b_{c}"], g[f"b_{c}_valid"]) for c in "ads"]
+    pkeys = [(g[f"p_{c}"], g[f"p_{c}_valid"]) for c in "ads"]
+    nb, npb = len(g["b_a"]), len(g["p_a"])
+    assert [tuple(r) for r in g["inner"].tolist()] == P.hash_join(bkeys, pkeys, nb, npb, "inner")
+    assert len(g["inner"]) > 50 and len(g["anti"]) > 50, "the fixture should hold matches and misses"
+    assert [tuple(r) for r in g["left"].tolist()] == P.hash_join(bkeys, pkeys, nb, npb, "left")
+    assert g["semi"].tolist() == P.hash_join(bkeys, pkeys, nb, npb, "semi")
+    assert g["anti"].tolist() == P.hash_join(bkeys, pkeys, nb, npb, "anti")
+    pk = [(g["mp_k"], g["mp_k_valid"])]
+    for name in ("nulls", "empty", "mixed"):
+        bk = [(g[f"mb_{name}_k"], g[f"mb_{name}_k_valid"])]
+        m, mv = P.hash_join(bk, pk, len(bk[0][0]), len(pk[0][0]), "mark")
+        np.testing.assert_array_equal(mv, g[f"mark_{name}_valid"], err_msg=name)
+        np.testing.assert_array_equal(m[mv], g[f"mark_{name}"][mv].astype(bool), err_msg=name)
+
+
+EDGE_WORDS = [0, 1, 2 ** 32 - 1, 2 ** 32, 2 ** 63, 2 ** 63 - 1, 2 ** 64 - 1, 0xD6E8FEB86659FD93]
+
+
+def test_murmur64_inverse_round_trips():
+    rng = np.random.default_rng(3)
+    words = EDGE_WORDS + [int(x) for x in rng.integers(0, 2 ** 64, size=1000, dtype=np.uint64)]
+    arr = np.array(words, dtype=np.uint64)
+    inv = np.array([P.murmur64_inverse(int(w)) for w in words], dtype=np.uint64)
+    np.testing.assert_array_equal(P.murmur64(inv), arr)
+    np.testing.assert_array_equal(np.array([P.murmur64_inverse(int(h)) for h in P.murmur64(arr)], dtype=np.uint64), arr)
+
+
+def test_combine_hash_preimage():
+    """a key constructed for a target hash reaches it through hash_columns, for BIGINT and UBIGINT last columns and
+    for the targets the join tests need: another key's full hash, and the table's empty-slot key 2^63"""
+    rng = np.random.default_rng(4)
+    a = rng.integers(-10 ** 9, 10 ** 9, size=64).astype(np.int64)
+    d = rng.standard_normal(64)
+    d[:3] = [0.0, -0.0, np.nan]
+    av = rng.random(64) > 0.2
+    prefix = P.hash_columns([(a, av), (d, None)])
+    targets = [2 ** 63, 0, 2 ** 64 - 1] + [int(x) for x in rng.integers(0, 2 ** 64, size=61, dtype=np.uint64)]
+    b = np.array([P.combine_hash_preimage(int(p), t) for p, t in zip(prefix, targets)], dtype=np.uint64)
+    for last in (b, b.view(np.int64)):
+        h = P.hash_columns([(a, av), (d, None), (last, None)])
+        assert [int(x) for x in h] == targets
+    # one column: the key itself is murmur64's preimage
+    assert int(P.hash_columns([(np.array([P.murmur64_inverse(2 ** 63)], dtype=np.uint64), None)])[0]) == 2 ** 63
+
+
 def test_radix_partition_ids():
     h = np.array([0, 1 << 45, 7 << 45, (1 << 48) - 1, 0xFFFF000000000000], dtype=np.uint64)
     np.testing.assert_array_equal(P.radix_partition_ids(h, 3), [0, 1, 7, 7, 0])
