@@ -69,6 +69,11 @@ struct b200_agg {
 	bool aos_empty;               // every group lives in `hc` (the generic table was emptied into it): finalize reads hc
 	PrivDirect priv_direct;       // PRIV path: direct slot addressing tables (nslots == 0: directory lookup instead)
 	void *priv_direct_dev;
+	// group count of the generic table as the last read_counters saw it; valid while counts_fresh, which that read sets
+	// and every call that enqueues work able to add groups or set the overflow flag clears (sink, combine_states,
+	// combine_packed, fix_cnt, growth, the merge of the high-cardinality table)
+	uint64_t last_groups;
+	bool counts_fresh;
 };
 
 // packed key word 0 of every group (PRIV's direct addressing tables are built from them)
@@ -497,6 +502,7 @@ static int agg_grow(b200_agg *agg, uint64_t min_capacity) {
 	B200_TRY(agg_alloc_table(agg, new_cap, &new_slots));
 	uint64_t *old_slots = agg->slots;
 	uint64_t old_cap = agg->capacity;
+	agg->counts_fresh = false;
 	agg->slots = new_slots;
 	agg->capacity = new_cap;
 	AggTable T = agg_table(agg);
@@ -670,6 +676,8 @@ static int read_counters(b200_agg *agg, uint64_t *groups, uint64_t *deferred, ui
 		               "b200_agg_export_states / the radix shuffle for this cardinality");
 		return B200_ERR_CAPACITY;
 	}
+	agg->last_groups = ctx->pinned_scratch[16];
+	agg->counts_fresh = true;
 	if (groups) {
 		*groups = ctx->pinned_scratch[16];
 	}
@@ -680,6 +688,28 @@ static int read_counters(b200_agg *agg, uint64_t *groups, uint64_t *deferred, ui
 		*missed = ctx->pinned_scratch[18];
 	}
 	return B200_OK;
+}
+
+// group count of the generic table: the last read_counters' value when nothing has been enqueued on the table since,
+// else a new read (one host round trip)
+static int agg_groups(b200_agg *agg, uint64_t *groups) {
+	if (agg->counts_fresh) {
+		*groups = agg->last_groups;
+		return B200_OK;
+	}
+	return read_counters(agg, groups, nullptr, nullptr);
+}
+
+// cnt(x) of input i starts being tracked: bring it up to date in every existing group
+static void agg_fix_cnt(b200_agg *agg, int i) {
+	b200_ctx *ctx = agg->ctx;
+	if (agg->rows_seen) {
+		int grid = grid_for(agg->capacity, 256, 4, ctx->sm_count * 8);
+		agg_fix_cnt_kernel<<<grid, 256, 0, ctx->stream>>>(agg->slots, agg->capacity, agg->L, i);
+		ctx->launches++;
+		agg->counts_fresh = false;
+	}
+	agg->track_cnt[i] = true;
 }
 
 // Run `launch(rows, begin, end, deferred, first)` until no row is deferred, growing the table in between.
@@ -752,7 +782,7 @@ static int agg_flush_hc(b200_agg *agg) {
 	b200_ctx *ctx = agg->ctx;
 	uint64_t hg = 0, groups = 0;
 	B200_TRY(b200_agg_hc_groups(ctx, agg->hc, &hg));
-	B200_TRY(read_counters(agg, &groups, nullptr, nullptr));
+	B200_TRY(agg_groups(agg, &groups));
 	uint64_t need = 2 * (groups + hg) + 16;
 	if (agg->capacity < need) {
 		B200_TRY(agg_grow(agg, need));
@@ -763,6 +793,7 @@ static int agg_flush_hc(b200_agg *agg) {
 		ac.track_cnt[i] = agg->track_cnt[i];
 	}
 	int rc = b200_agg_hc_flush(ctx, agg->hc, agg->L, agg_table(agg), ac);
+	agg->counts_fresh = false;
 	b200_agg_hc_destroy(ctx, agg->hc);
 	agg->hc = nullptr;
 	agg->aos_empty = false;
@@ -816,6 +847,35 @@ static int agg_build_priv_direct(b200_agg *agg, uint64_t groups, int max_slots) 
 	return B200_OK;
 }
 
+// A finalize result block of at most this many bytes is copied to the host whole, once, at finalize, and
+// b200_batch_download serves it from that copy.  Larger results stay on the device until a column is downloaded: a
+// 1 M-group result (TPC-H Q3, about 27 MB) would otherwise pay a ~1 ms copy inside every finalize, also when the
+// caller keeps the result on the device or reads only part of it.  The Q1 and SSB results are a few hundred bytes.
+#define AGG_RESULT_HOST_COPY_MAX ((size_t)1 << 20)
+
+// bytes one result column takes in the block: 16-byte aligned, with 16 bytes of slack
+static size_t result_span(size_t bytes) {
+	return (bytes + 16 + 15) & ~(size_t)15;
+}
+
+// integer AVG: finish on the host in long double, bit-exact with
+// IntegerAverageOperationHugeint::Finalize (avg.cpp:109-121): Hugeint::Cast<long double>(sum) / count
+static void avg_finish(int in_type, const uint64_t *raw, double *res, uint64_t groups) {
+	bool is_signed = b200_type_is_signed_int(in_type);
+	for (uint64_t g = 0; g < groups; g++) {
+		uint64_t lo = raw[3 * g], hi = raw[3 * g + 1], cnt = raw[3 * g + 2];
+		long double v;
+		if (is_signed && (int64_t)hi < 0) {
+			// negate the 128-bit value, convert, negate (Hugeint::Cast<long double>)
+			uint64_t nlo = ~lo + 1, nhi = ~hi + (nlo == 0 ? 1 : 0);
+			v = -((long double)nhi * 18446744073709551616.0L + (long double)nlo);
+		} else {
+			v = (long double)hi * 18446744073709551616.0L + (long double)lo;
+		}
+		res[g] = cnt ? (double)(v / (long double)cnt) : 0.0;
+	}
+}
+
 extern "C" {
 
 int b200_agg_sink(b200_agg *agg, const b200_batch *in, const int *key_cols, const int *input_cols) {
@@ -857,15 +917,11 @@ int b200_agg_sink(b200_agg *agg, const b200_batch *in, const int *key_cols, cons
 		return B200_ERR_INVALID;
 	}
 	CUDA_TRY(cudaSetDevice(ctx->device));
+	agg->counts_fresh = false;
 	// inputs that arrive with a validity mask for the first time: start tracking cnt(x)
 	for (int i = 0; i < L.ninputs; i++) {
 		if (ac.c[i].validity && !agg->track_cnt[i]) {
-			if (agg->rows_seen) {
-				int grid = grid_for(agg->capacity, 256, 4, ctx->sm_count * 8);
-				agg_fix_cnt_kernel<<<grid, 256, 0, ctx->stream>>>(agg->slots, agg->capacity, L, i);
-				ctx->launches++;
-			}
-			agg->track_cnt[i] = true;
+			agg_fix_cnt(agg, i);
 		}
 		ac.track_cnt[i] = agg->track_cnt[i];
 	}
@@ -894,7 +950,7 @@ int b200_agg_sink(b200_agg *agg, const b200_batch *in, const int *key_cols, cons
 			}
 			if (!agg->hc) {
 				uint64_t g0 = 0;
-				B200_TRY(read_counters(agg, &g0, nullptr, nullptr));
+				B200_TRY(agg_groups(agg, &g0));
 				uint64_t hint = 2 * (uint64_t)agg->path_groups_hc;
 				B200_TRY(b200_agg_hc_prepare(ctx, &agg->hc, L, agg->track_cnt, hint > 2 * g0 ? hint : 2 * g0));
 				// the groups the generic table already holds (the adaptation probe's rows) move into the new table: from
@@ -905,6 +961,7 @@ int b200_agg_sink(b200_agg *agg, const b200_batch *in, const int *key_cols, cons
 					agg_init_kernel<<<grid, 256, 0, ctx->stream>>>(agg->slots, agg->capacity, L);
 					ctx->launches++;
 					CUDA_TRY(cudaMemsetAsync(agg->count, 0, 8, ctx->stream));
+					agg->counts_fresh = false;
 				}
 				agg->aos_empty = true;
 			}
@@ -977,9 +1034,10 @@ int b200_agg_sink(b200_agg *agg, const b200_batch *in, const int *key_cols, cons
 		if (path != PATH_GLOBAL && !agg->path_decided) {
 			// adaptation (the analogue of DecideAdaptation's HyperLogLog estimate): every row of the probe chunk has
 			// been aggregated - in shared memory or, on a miss, inline in the global table - so the table's group
-			// count is the exact cardinality of the first rows.  Pick the cheapest structure that holds it.
+			// count is the exact cardinality of the first rows.  Pick the cheapest structure that holds it.  (The count
+			// came back with run_with_growth's last read.)
 			uint64_t groups = 0;
-			B200_TRY(read_counters(agg, &groups, nullptr, nullptr));
+			B200_TRY(agg_groups(agg, &groups));
 			const char *priv_env = getenv("B200_AGG_PRIV"); // experiment knob: 0 = never PRIV, 2 = PRIV also for <= 8 groups
 			int priv_mode = priv_env ? atoi(priv_env) : 1;
 			int priv_cap = priv_mode ? b200_agg_priv_capacity(L) : 0;
@@ -1018,7 +1076,7 @@ int b200_agg_group_count(b200_agg *agg, uint64_t *out_groups) {
 		return b200_agg_hc_groups(agg->ctx, agg->hc, out_groups);
 	}
 	B200_TRY(agg_flush_hc(agg));
-	return read_counters(agg, out_groups, nullptr, nullptr);
+	return agg_groups(agg, out_groups);
 }
 
 int b200_agg_finalize(b200_agg *agg, b200_batch **out) {
@@ -1032,45 +1090,72 @@ int b200_agg_finalize(b200_agg *agg, b200_batch **out) {
 	const bool from_hc = agg->hc && agg->aos_empty; // every group lives in the high-cardinality table: read it directly
 	uint64_t groups = 0;
 	if (from_hc) {
-		B200_TRY(read_counters(agg, nullptr, nullptr, nullptr)); // (reports a packed-buffer overflow, if any)
+		if (!agg->counts_fresh) {
+			B200_TRY(read_counters(agg, nullptr, nullptr, nullptr)); // (reports a packed-buffer overflow, if any)
+		}
 		B200_TRY(b200_agg_hc_groups(ctx, agg->hc, &groups));
 	} else {
 		B200_TRY(agg_flush_hc(agg));
-		B200_TRY(read_counters(agg, &groups, nullptr, nullptr));
+		B200_TRY(agg_groups(agg, &groups));
 	}
+	// ONE device block holds the whole result: [key columns | aggregate columns | integer-AVG triples | validity words
+	// of every column].  Each column starts 16-byte aligned and has 16 bytes of slack, as b200_batch_add_flat gives one.
+	const int ncols = L.nkeys + L.naggs;
+	const uint64_t vwords = ((groups + 63) / 64 + 2) & ~(uint64_t)1; // per column: >= 1 spare word, 16-byte multiple
+	size_t data_off[MAX_KEYS + MAX_AGGS], triple_off[MAX_AGGS];
+	int type[MAX_KEYS + MAX_AGGS];
+	size_t off = 0;
+	for (int c = 0; c < ncols; c++) {
+		type[c] = c < L.nkeys ? L.key_type[c] : agg_result_type(L.func[c - L.nkeys], L.in_type[c - L.nkeys]);
+		data_off[c] = off;
+		off += result_span((size_t)groups * b200_type_size(type[c]));
+	}
+	size_t avg_lo = 0, avg_hi = 0; // bytes of the block that hold the integer-AVG result columns
+	for (int a = 0; a < L.naggs; a++) {
+		triple_off[a] = 0;
+		if (L.func[a] == B200_AGG_AVG && !b200_type_is_float(L.in_type[a])) {
+			triple_off[a] = off; // the kernel writes raw [lo, hi, count] triples here; the host finishes the column
+			off += result_span((size_t)groups * 24);
+			size_t lo = data_off[L.nkeys + a], hi = lo + (size_t)groups * 8;
+			avg_lo = avg_hi == 0 || lo < avg_lo ? lo : avg_lo;
+			avg_hi = hi > avg_hi ? hi : avg_hi;
+		}
+	}
+	const size_t valid_off = off;
+	const size_t block_bytes = valid_off + (size_t)ncols * vwords * 8;
+	void *block = nullptr;
+	B200_TRY(b200_dev_alloc(ctx, block_bytes, &block));
 	b200_batch *ob = b200_batch_new(ctx, groups);
+	ob->owned.push_back(block);
+	uint8_t *base = (uint8_t *)block;
+	uint64_t *valid = (uint64_t *)(base + valid_off);
 	FinalizeOut fo;
 	memset(&fo, 0, sizeof(fo));
 	for (int i = 0; i < L.ninputs; i++) {
 		fo.track_cnt[i] = agg->track_cnt[i];
 	}
-	uint64_t words = (groups + 63) / 64;
-	int rc = B200_OK;
-	for (int j = 0; j < L.nkeys && rc == B200_OK; j++) {
-		rc = b200_batch_add_flat(ob, L.key_type[j], groups, true, &fo.key_data[j], &fo.key_valid[j]);
-		if (rc == B200_OK && words) {
-			fill_u64_kernel3<<<grid_for(words, 256, 1, 1024), 256, 0, ctx->stream>>>(fo.key_valid[j], words, ~0ULL);
-			ctx->launches++;
+	for (int c = 0; c < ncols; c++) {
+		DCol col;
+		col.data = base + data_off[c];
+		col.sel = nullptr;
+		col.validity = valid + c * vwords;
+		col.type = type[c];
+		col.vtype = B200_FLAT_VECTOR;
+		ob->cols.push_back(col);
+		ob->dict_sizes.push_back(0);
+		if (c < L.nkeys) {
+			fo.key_data[c] = base + data_off[c];
+			fo.key_valid[c] = valid + c * vwords;
+		} else {
+			int a = c - L.nkeys;
+			fo.agg_data[a] = triple_off[a] ? base + triple_off[a] : base + data_off[c];
+			fo.agg_valid[a] = valid + c * vwords;
 		}
 	}
-	std::vector<void *> avg_raw(L.naggs, nullptr);
-	for (int a = 0; a < L.naggs && rc == B200_OK; a++) {
-		int rt = agg_result_type(L.func[a], L.in_type[a]);
-		rc = b200_batch_add_flat(ob, rt, groups, true, &fo.agg_data[a], &fo.agg_valid[a]);
-		if (rc == B200_OK && words) {
-			fill_u64_kernel3<<<grid_for(words, 256, 1, 1024), 256, 0, ctx->stream>>>(fo.agg_valid[a], words, ~0ULL);
-			ctx->launches++;
-		}
-		if (rc == B200_OK && L.func[a] == B200_AGG_AVG && !b200_type_is_float(L.in_type[a])) {
-			rc = b200_dev_alloc(ctx, (size_t)groups * 24 + 16, &avg_raw[a]);
-			if (rc == B200_OK) {
-				std::swap(fo.agg_data[a], avg_raw[a]); // kernel writes raw triples; column filled by the host
-			}
-		}
-	}
-	if (rc != B200_OK) {
-		b200_batch_free(ob);
-		return rc;
+	if (groups) {
+		// every validity word of the result at once (all valid; the finalize kernel clears the NULL bits)
+		fill_u64_kernel3<<<grid_for(ncols * vwords, 256, 1, 1024), 256, 0, ctx->stream>>>(valid, ncols * vwords, ~0ULL);
+		ctx->launches++;
 	}
 	unsigned long long *out_counter = agg->counters + 2;
 	cudaMemsetAsync(out_counter, 0, 8, ctx->stream);
@@ -1085,59 +1170,78 @@ int b200_agg_finalize(b200_agg *agg, b200_batch **out) {
 		agg_finalize_kernel<<<grid, 256, 0, ctx->stream>>>(agg->slots, agg->capacity, L, fo, out_counter);
 		ctx->launches++;
 	}
-	// integer AVG: finish on the host in long double, bit-exact with
-	// IntegerAverageOperationHugeint::Finalize (avg.cpp:109-121): Hugeint::Cast<long double>(sum) / count
-	for (int a = 0; a < L.naggs; a++) {
-		if (!avg_raw[a]) {
+	cudaError_t e = cudaSuccess;
+	if (block_bytes <= AGG_RESULT_HOST_COPY_MAX) {
+		// small result: the whole block to the host in one copy and one synchronise; the integer AVGs are finished in
+		// the host copy, and one copy puts them back into the device block (which stays a valid device view)
+		int rc = b200_host_alloc(ctx, block_bytes, &ob->host);
+		if (rc != B200_OK) {
+			b200_batch_free(ob);
+			return rc;
+		}
+		uint8_t *hbase = (uint8_t *)ob->host;
+		e = cudaMemcpyAsync(hbase, base, block_bytes, cudaMemcpyDeviceToHost, ctx->stream);
+		e = e ? e : cudaStreamSynchronize(ctx->stream);
+		e = e ? e : cudaGetLastError();
+		if (e != cudaSuccess) {
+			b200_batch_free(ob);
+			return b200_cuda_fail(e, "agg_finalize (D2H of the result)", __FILE__, __LINE__);
+		}
+		ctx->d2h_bytes += block_bytes;
+		for (int c = 0; c < ncols; c++) {
+			ob->host_data.push_back(hbase + data_off[c]);
+			ob->host_valid.push_back((const uint64_t *)(hbase + valid_off) + c * vwords);
+		}
+		for (int a = 0; a < L.naggs; a++) {
+			if (triple_off[a]) {
+				avg_finish(L.in_type[a], (const uint64_t *)(hbase + triple_off[a]), (double *)(hbase + data_off[L.nkeys + a]),
+				           groups);
+			}
+		}
+		if (groups && avg_hi) {
+			// (the other columns inside [avg_lo, avg_hi) are copied back unchanged)
+			e = cudaEventCreateWithFlags(&ob->host_done, cudaEventDisableTiming);
+			e = e ? e : cudaMemcpyAsync(base + avg_lo, hbase + avg_lo, avg_hi - avg_lo, cudaMemcpyHostToDevice, ctx->stream);
+			e = e ? e : cudaEventRecord(ob->host_done, ctx->stream);
+			if (e != cudaSuccess) {
+				b200_batch_free(ob);
+				return b200_cuda_fail(e, "agg_finalize (H2D of the averages)", __FILE__, __LINE__);
+			}
+			ctx->h2d_bytes += avg_hi - avg_lo;
+		}
+		*out = ob;
+		return B200_OK;
+	}
+	// large result: stays on the device; each integer AVG's triples make one round trip through pinned staging
+	void *stage = nullptr;
+	if (groups && avg_hi) {
+		int rc = b200_host_alloc(ctx, (size_t)groups * 32, &stage);
+		if (rc != B200_OK) {
+			b200_batch_free(ob);
+			return rc;
+		}
+	}
+	uint64_t *raw = (uint64_t *)stage;
+	double *res = (double *)(raw + 3 * groups);
+	for (int a = 0; a < L.naggs && stage && e == cudaSuccess; a++) {
+		if (!triple_off[a]) {
 			continue;
 		}
-		void *raw_dev = fo.agg_data[a];
-		void *col_dev = avg_raw[a];
-		std::vector<uint64_t> raw(groups * 3);
-		std::vector<double> res(groups);
-		if (groups) {
-			cudaError_t e = cudaMemcpyAsync(raw.data(), raw_dev, groups * 24, cudaMemcpyDeviceToHost, ctx->stream);
-			e = e ? e : cudaStreamSynchronize(ctx->stream);
-			if (e != cudaSuccess) {
-				for (int q = a; q < L.naggs; q++) {
-					if (avg_raw[q]) {
-						b200_dev_free(ctx, fo.agg_data[q]); // the raw triples of the averages not finished yet
-					}
-				}
-				b200_batch_free(ob);
-				return b200_cuda_fail(e, "avg finalize D2H", __FILE__, __LINE__);
-			}
-			ctx->d2h_bytes += groups * 24;
-			bool is_signed = b200_type_is_signed_int(L.in_type[a]);
-			for (uint64_t g = 0; g < groups; g++) {
-				uint64_t lo = raw[3 * g], hi = raw[3 * g + 1], cnt = raw[3 * g + 2];
-				long double v;
-				if (is_signed && (int64_t)hi < 0) {
-					// negate the 128-bit value, convert, negate (Hugeint::Cast<long double>)
-					uint64_t nlo = ~lo + 1, nhi = ~hi + (nlo == 0 ? 1 : 0);
-					v = -((long double)nhi * 18446744073709551616.0L + (long double)nlo);
-				} else {
-					v = (long double)hi * 18446744073709551616.0L + (long double)lo;
-				}
-				res[g] = cnt ? (double)(v / (long double)cnt) : 0.0;
-			}
-			e = cudaMemcpyAsync(col_dev, res.data(), groups * 8, cudaMemcpyHostToDevice, ctx->stream);
-			e = e ? e : cudaStreamSynchronize(ctx->stream);
-			if (e != cudaSuccess) {
-				for (int q = a; q < L.naggs; q++) {
-					if (avg_raw[q]) {
-						b200_dev_free(ctx, fo.agg_data[q]);
-					}
-				}
-				b200_batch_free(ob);
-				return b200_cuda_fail(e, "avg finalize H2D", __FILE__, __LINE__);
-			}
-			ctx->h2d_bytes += groups * 8;
+		// (the previous average's H2D from `res` is ordered before this D2H, so the host writes `res` only after it)
+		e = cudaMemcpyAsync(raw, base + triple_off[a], groups * 24, cudaMemcpyDeviceToHost, ctx->stream);
+		e = e ? e : cudaStreamSynchronize(ctx->stream);
+		if (e != cudaSuccess) {
+			break;
 		}
-		b200_dev_free(ctx, raw_dev);
+		ctx->d2h_bytes += groups * 24;
+		avg_finish(L.in_type[a], raw, res, groups);
+		e = cudaMemcpyAsync(base + data_off[L.nkeys + a], res, groups * 8, cudaMemcpyHostToDevice, ctx->stream);
+		ctx->h2d_bytes += groups * 8;
 	}
-	cudaError_t e = cudaStreamSynchronize(ctx->stream);
+	cudaError_t e2 = cudaStreamSynchronize(ctx->stream);
+	e = e ? e : e2;
 	e = e ? e : cudaGetLastError();
+	b200_host_free(ctx, stage);
 	if (e != cudaSuccess) {
 		b200_batch_free(ob);
 		return b200_cuda_fail(e, "agg_finalize", __FILE__, __LINE__);
@@ -1156,7 +1260,7 @@ int b200_agg_export_states(b200_agg *agg, b200_batch **out) {
 	CUDA_TRY(cudaSetDevice(ctx->device));
 	B200_TRY(agg_flush_hc(agg));
 	uint64_t groups = 0;
-	B200_TRY(read_counters(agg, &groups, nullptr, nullptr));
+	B200_TRY(agg_groups(agg, &groups));
 	b200_batch *ob = b200_batch_new(ctx, groups);
 	ExportOut eo;
 	memset(&eo, 0, sizeof(eo));
@@ -1242,15 +1346,11 @@ int b200_agg_combine_states(b200_agg *agg, const b200_batch *states) {
 	}
 	CUDA_TRY(cudaSetDevice(ctx->device));
 	B200_TRY(agg_flush_hc(agg));
+	agg->counts_fresh = false;
 	// exported states carry an explicit cnt(x) for every input: from now on cnt is tracked here as well
 	for (int i = 0; i < L.ninputs; i++) {
 		if (!agg->track_cnt[i]) {
-			if (agg->rows_seen) {
-				int grid = grid_for(agg->capacity, 256, 4, ctx->sm_count * 8);
-				agg_fix_cnt_kernel<<<grid, 256, 0, ctx->stream>>>(agg->slots, agg->capacity, L, i);
-				ctx->launches++;
-			}
-			agg->track_cnt[i] = true;
+			agg_fix_cnt(agg, i);
 		}
 	}
 	agg->rows_seen += n;
@@ -1315,7 +1415,7 @@ int b200_agg_combine_packed(b200_agg *agg, const uint64_t *src_dev, int nranks, 
 	uint64_t incoming = (uint64_t)nranks * max_groups;
 	if (agg->rows_seen != 0) {
 		uint64_t groups = 0;
-		B200_TRY(read_counters(agg, &groups, nullptr, nullptr));
+		B200_TRY(agg_groups(agg, &groups));
 		incoming += groups;
 	}
 	if (agg->capacity < 2 * incoming + 16) {
@@ -1323,14 +1423,11 @@ int b200_agg_combine_packed(b200_agg *agg, const uint64_t *src_dev, int nranks, 
 	}
 	for (int i = 0; i < L.ninputs; i++) {
 		if (!agg->track_cnt[i]) {
-			if (agg->rows_seen) {
-				int grid = grid_for(agg->capacity, 256, 4, ctx->sm_count * 8);
-				agg_fix_cnt_kernel<<<grid, 256, 0, ctx->stream>>>(agg->slots, agg->capacity, L, i);
-				ctx->launches++;
-			}
-			agg->track_cnt[i] = true;
+			agg_fix_cnt(agg, i);
 		}
 	}
+	// the merge below adds groups and may set the overflow flag: the next finalize reads the counters again
+	agg->counts_fresh = false;
 	agg->rows_seen += 1;
 	StateMap sm;
 	state_map(L, &sm);

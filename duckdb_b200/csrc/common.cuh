@@ -67,6 +67,14 @@ struct b200_batch {
 	std::vector<DCol> cols;
 	std::vector<uint64_t> dict_sizes;
 	std::vector<void *> owned; // device allocations freed with the batch
+	// A small finalize result (b200_agg_finalize) also has a pinned host copy of its device block, taken once at
+	// finalize: b200_batch_download serves every column from it.  host_data[i] / host_valid[i] are cols[i]'s data /
+	// validity in that copy.  host_done, when set, is recorded after the last copy that reads the host copy;
+	// b200_batch_free waits for it before the buffer goes back to the b200_host_alloc cache.
+	void *host = nullptr;
+	std::vector<const void *> host_data;
+	std::vector<const uint64_t *> host_valid;
+	cudaEvent_t host_done = nullptr;
 };
 
 int b200_dev_alloc(b200_ctx *ctx, size_t bytes, void **out);

@@ -560,8 +560,23 @@ int b200_batch_download(b200_ctx *ctx, const b200_batch *b, int col, void *dst_d
 		b200_set_error("b200_batch_download: only flat columns can be downloaded");
 		return B200_ERR_INVALID;
 	}
-	CUDA_TRY(cudaSetDevice(ctx->device));
 	size_t bytes = (size_t)b->nrows * b200_type_size(c.type);
+	if (b->host) {
+		// a small finalize result: served from the host copy taken at finalize, no CUDA call
+		size_t words = (b->nrows + 63) / 64;
+		if (dst_data && bytes) {
+			memcpy(dst_data, b->host_data[col], bytes);
+		}
+		if (dst_validity && words) {
+			if (b->host_valid[col]) {
+				memcpy(dst_validity, b->host_valid[col], words * 8);
+			} else {
+				memset(dst_validity, 0xff, words * 8);
+			}
+		}
+		return B200_OK;
+	}
+	CUDA_TRY(cudaSetDevice(ctx->device));
 	if (dst_data && bytes) {
 		CUDA_TRY(cudaMemcpyAsync(dst_data, c.data, bytes, cudaMemcpyDeviceToHost, ctx->stream));
 		ctx->d2h_bytes += bytes;
@@ -589,6 +604,13 @@ void b200_batch_free(b200_batch *b) {
 		return;
 	}
 	cudaSetDevice(b->ctx->device);
+	if (b->host_done) {
+		cudaEventSynchronize(b->host_done); // a copy from the host copy may still be in flight
+		cudaEventDestroy(b->host_done);
+	}
+	if (b->host) {
+		b200_host_free(b->ctx, b->host);
+	}
 	for (void *p : b->owned) {
 		b200_dev_free(b->ctx, p);
 	}

@@ -131,7 +131,8 @@ B200_API uint64_t b200_batch_rows(const b200_batch *b);
 B200_API int b200_batch_cols(const b200_batch *b);
 /* device view of column i (pointers are device pointers). */
 B200_API int b200_batch_column(const b200_batch *b, int col, b200_vector *out);
-/* copy column data (flat values) / validity words of column i back to host. */
+/* copy column data (flat values) / validity words of column i back to host.  A result of b200_agg_finalize of at
+ * most 1 MiB is served from the pinned host copy finalize took of it: a memcpy, no CUDA call. */
 B200_API int b200_batch_download(b200_ctx *ctx, const b200_batch *b, int col, void *dst_data,
                                  uint64_t *dst_validity);
 B200_API void b200_batch_free(b200_batch *b);
@@ -292,6 +293,10 @@ B200_API int b200_agg_combine_packed(b200_agg *agg, const uint64_t *src_dev, int
  * (physical_hash_aggregate.hpp:110-112).  Result types: COUNT* -> INT64;
  * SUM(int) -> INT128; SUM_NO_OVERFLOW -> INT64; SUM(float/double) -> DOUBLE;
  * MIN/MAX -> input type; AVG -> DOUBLE.
+ * The result is read-only: its columns share one device block, and a result of
+ * at most 1 MiB also has a host copy taken at finalize, from which
+ * b200_batch_download serves it (writes through b200_batch_column pointers
+ * would not reach that copy).
  * Replaces RadixPartitionedHashTable::GetData / RowOperations::FinalizeStates
  * (radix_partitioned_hashtable.cpp:1307-1360,1374-1442). */
 B200_API int b200_agg_finalize(b200_agg *agg, b200_batch **out);
