@@ -936,20 +936,6 @@ static bool col_stageable(const DCol &c) {
 	return true;
 }
 
-int b200_agg_tile_eligible(const AggLayout &L, const KeyCols &keys, const AggCols &ac) {
-	for (int j = 0; j < L.nkeys; j++) {
-		if (!col_stageable(keys.c[j])) {
-			return B200_ERR_INVALID;
-		}
-	}
-	for (int i = 0; i < L.ninputs; i++) {
-		if (!col_stageable(ac.c[i])) {
-			return B200_ERR_INVALID;
-		}
-	}
-	return B200_OK; // (key width limits of the individual paths are checked by b200_agg_sink)
-}
-
 static int add_tile_col(TileCols *tc, const void *ptr, uint32_t width) {
 	// the same column may be referenced several times (key and input, or two inputs): stage it once
 	for (int i = 0; i < tc->n; i++) {
@@ -963,6 +949,26 @@ static int add_tile_col(TileCols *tc, const void *ptr, uint32_t width) {
 	tc->c[tc->n].ptr = (const unsigned char *)ptr;
 	tc->c[tc->n].width = width;
 	return tc->n++;
+}
+
+int b200_agg_tile_eligible(const AggLayout &L, const KeyCols &keys, const AggCols &ac) {
+	// every distinct data and validity column takes a slot of the stage: DuckDB hands each aggregate its own copy of
+	// the input column, so ten aggregates over two nullable inputs already stage 20 columns besides the keys
+	TileCols tc;
+	tc.n = 0;
+	for (int j = 0; j < L.nkeys; j++) {
+		if (!col_stageable(keys.c[j]) || add_tile_col(&tc, keys.c[j].data, b200_type_size(keys.c[j].type)) < 0 ||
+		    (keys.c[j].validity && add_tile_col(&tc, keys.c[j].validity, 0) < 0)) {
+			return B200_ERR_INVALID;
+		}
+	}
+	for (int i = 0; i < L.ninputs; i++) {
+		if (!col_stageable(ac.c[i]) || add_tile_col(&tc, ac.c[i].data, b200_type_size(ac.c[i].type)) < 0 ||
+		    (ac.c[i].validity && add_tile_col(&tc, ac.c[i].validity, 0) < 0)) {
+			return B200_ERR_INVALID;
+		}
+	}
+	return B200_OK; // (key width limits of the individual paths are checked by b200_agg_sink)
 }
 
 // upper bound on the groups one launch can add to the global table through the end-of-CTA flushes

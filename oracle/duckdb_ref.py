@@ -192,23 +192,27 @@ class Connection:
                     buf = (C.c_char * (n * 16)).from_address(data) if n else b""
                     raw = np.frombuffer(buf, dtype=np.uint64, count=2 * n).copy().reshape(n, 2)
                     # python ints: upper is signed
-                    vals = np.array([int(lo) + (int(np.array(hi).astype(np.int64)) << 64) for lo, hi in raw],
-                                    dtype=object)
+                    vals = raw[:, 1].astype(np.int64).astype(object) * (1 << 64) + raw[:, 0].astype(object)
                     parts[i].append(vals)
                 elif ph == T_VARCHAR:
-                    out = []
-                    for r in range(n):
-                        if not bits[r]:
-                            out.append(None)
-                            continue
-                        base = data + r * 16
-                        ln = C.c_uint32.from_address(base).value
+                    # string_t: 4-byte length, then up to 12 inlined bytes or a 4-byte prefix and a pointer
+                    raw = np.frombuffer((C.c_char * (n * 16)).from_address(data), dtype=np.uint8).reshape(n, 16) \
+                        if n else np.zeros((0, 16), np.uint8)
+                    lens = raw[:, :4].copy().view(np.uint32)[:, 0]
+                    inlined = np.frombuffer(raw[:, 4:].tobytes(), dtype="S12")  # trailing NUL bytes dropped
+                    # all at once where the bytes after the string are zero, so the S12 value is the string
+                    fast = bits & (lens <= 12) & (np.char.str_len(inlined) == lens)
+                    out = np.empty(n, dtype=object)
+                    out[fast] = [s.decode("utf8", "replace") for s in inlined[fast].tolist()]
+                    for r in np.flatnonzero(bits & ~fast):
+                        base = data + int(r) * 16
+                        ln = int(lens[r])
                         if ln <= 12:
-                            out.append(C.string_at(base + 4, ln).decode("utf8", "replace"))
+                            out[r] = C.string_at(base + 4, ln).decode("utf8", "replace")
                         else:
                             ptr = C.c_void_p.from_address(base + 8).value
-                            out.append(C.string_at(ptr, ln).decode("utf8", "replace"))
-                    parts[i].append(np.array(out, dtype=object))
+                            out[r] = C.string_at(ptr, ln).decode("utf8", "replace")
+                    parts[i].append(out)
                 else:
                     raise RuntimeError(f"unsupported result type {ph} for column {names[i]}")
             L.duckdb_destroy_data_chunk(C.byref(chunk))

@@ -25,11 +25,13 @@ KERNEL_CASES = {
     "agg_fast_kernel": ["test_fast_kernel_shapes", "test_fast_partial_overflow", "test_minmax_type_limits"],
     "agg_priv_kernel": ["test_ubigint_sum_near_2_64", "test_priv_kernels", "test_priv_direct_edges"],
     "agg_wpriv_kernel": ["test_ubigint_sum_near_2_64", "test_priv_kernels", "test_priv_direct_edges"],
-    "agg_mid_kernel": ["test_mid_kernel", "test_mid_spill", "test_minmax_type_limits"],
+    "agg_mid_kernel": ["test_mid_kernel", "test_mid_spill", "test_minmax_type_limits",
+                       "test_more_columns_than_a_tile_stage_takes"],
     "agg_mid2_kernel": ["test_ubigint_sum_near_2_64", "test_mid2_kernel", "test_mid2_periodic_flushes"],
     "agg_list_keys_kernel": ["test_priv_kernels"],
     "agg_init_kernel": ["test_generic_table_growth_and_replay"],
-    "agg_sink_kernel": ["test_generic_table_growth_and_replay", "test_mid_not_for_long_keys"],
+    "agg_sink_kernel": ["test_generic_table_growth_and_replay", "test_mid_not_for_long_keys",
+                        "test_more_columns_than_a_tile_stage_takes"],
     "agg_rehash_kernel": ["test_generic_table_growth_and_replay"],
     "agg_fix_cnt_kernel": ["test_validity_arrives_later"],
     "agg_finalize_kernel": ["test_generic_table_growth_and_replay"],
@@ -606,6 +608,27 @@ def test_mid_kernel(ctx, shape):
     names = agg_run(ctx, keys, gid, ng, inputs, aggs)
     assert_ran(names, "agg_mid_kernel")
     assert_not_ran(names, "agg_priv_kernel", "agg_wpriv_kernel", "agg_fastreg_kernel", "agg_mid2_kernel")
+
+
+@pytest.mark.parametrize("ninputs", [9, 10])
+def test_more_columns_than_a_tile_stage_takes(ctx, ninputs):
+    """DuckDB hands every aggregate its own copy of the input column, so ten aggregates over nullable inputs with a
+    nullable key stage 22 columns, two more than a tile stage holds (TP_MAX_COLS).  Such a batch must go to the
+    generic sink kernel: it used to be dispatched to the MID path, which refused it ("too many staged columns") and
+    failed the query.  Nine inputs (20 columns) still fit and take MID."""
+    rng = np.random.default_rng(ninputs)
+    n, ng = PROBE + 50_001, 35
+    gid = rng.integers(0, ng, size=n)
+    keys = [((gid * 7 - 100).astype(np.int32), gid != 0)]   # group 0 is the NULL key
+    inputs = [(rng.integers(-2 ** 31, 2 ** 31, size=n).astype(np.int32), rng.random(n) > 0.2) for _ in range(ninputs)]
+    aggs = [("sum", i) for i in range(ninputs)] + [("count", 0), ("min", 1), ("max", 2), ("avg", 3), ("count_star", -1)]
+    names = agg_run(ctx, keys, gid, ng, inputs, aggs)
+    if ninputs == 10:
+        assert_ran(names, "agg_sink_kernel")
+        assert_not_ran(names, "agg_mid_kernel", "agg_mid2_kernel", "agg_priv_kernel", "agg_wpriv_kernel",
+                       "agg_fastreg_kernel")
+    else:
+        assert_ran(names, "agg_mid_kernel")
 
 
 def test_mid_spill(ctx):
