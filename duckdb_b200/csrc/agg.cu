@@ -35,7 +35,7 @@ int b200_agg_priv_capacity(const AggLayout &L);
 struct AggHc;
 int b200_agg_hc_eligible(const AggLayout &L);
 int b200_agg_hc_prepare(b200_ctx *ctx, AggHc **hc_io, const AggLayout &L, const bool *track_cnt, uint64_t groups_hint);
-bool b200_agg_hc_compatible(const AggHc *hc, const AggLayout &L, const bool *track_cnt);
+bool b200_agg_hc_compatible(const AggHc *hc, const AggLayout &L, const bool *track_cnt, uint64_t rows);
 uint64_t b200_agg_hc_capacity(const AggHc *hc);
 int b200_agg_hc_groups(b200_ctx *ctx, AggHc *hc, uint64_t *groups);
 int b200_agg_hc_grow(b200_ctx *ctx, const AggLayout &L, AggHc *hc, uint64_t new_cap);
@@ -44,7 +44,7 @@ int b200_agg_hc_sink(b200_ctx *ctx, AggHc *hc, const AggLayout &L, const KeyCols
                      unsigned long long *counters);
 int b200_agg_hc_flush(b200_ctx *ctx, AggHc *hc, const AggLayout &L, const AggTable &T, const AggCols &ac);
 int b200_agg_hc_absorb(b200_ctx *ctx, AggHc *hc, const AggLayout &L, const uint64_t *slots, uint64_t capacity,
-                       const bool *track_cnt);
+                       const bool *track_cnt, uint64_t rows);
 int b200_agg_hc_finalize(b200_ctx *ctx, AggHc *hc, const AggLayout &L, const FinalizeOut &fo, unsigned long long *out_counter);
 void b200_agg_hc_destroy(b200_ctx *ctx, AggHc *hc);
 void b200_agg_hc_unpin(b200_ctx *ctx, AggHc *hc);
@@ -67,6 +67,10 @@ struct b200_agg {
 	uint64_t rows_seen;
 	AggHc *hc;                    // high-cardinality front-end table (merged into `slots` before any read-out)
 	bool aos_empty;               // every group lives in `hc` (the generic table was emptied into it): finalize reads hc
+	// rows the generic table's states hold while they all came from this aggregate's sinks; ~0 once a combine or the
+	// merge of a high-cardinality table has added sums of any size.  A new high-cardinality table absorbs the generic
+	// table only when these rows fit its lifetime: in practice, the adaptation probe's rows.
+	uint64_t generic_rows;
 	PrivDirect priv_direct;       // PRIV path: direct slot addressing tables (nslots == 0: directory lookup instead)
 	void *priv_direct_dev;
 	// group count of the generic table as the last read_counters saw it; valid while counts_fresh, which that read sets
@@ -797,6 +801,7 @@ static int agg_flush_hc(b200_agg *agg) {
 	b200_agg_hc_destroy(ctx, agg->hc);
 	agg->hc = nullptr;
 	agg->aos_empty = false;
+	agg->generic_rows = ~0ULL;
 	return rc;
 }
 
@@ -944,31 +949,37 @@ int b200_agg_sink(b200_agg *agg, const b200_batch *in, const int *key_cols, cons
 			// High cardinality: the L2-first table of agg_hc.cu.  Chunks of 1 M, 2 M, ... 16 M rows; a chunk whose rows
 			// find the table at its fill limit defers them, the table doubles and they are replayed; between chunks the
 			// table also doubles once it is more than 55 % full.  (Doubling, never more: the table should stay inside
-			// L2 for as long as the data allows.)
-			if (agg->hc && !b200_agg_hc_compatible(agg->hc, L, agg->track_cnt)) {
-				B200_TRY(agg_flush_hc(agg));
-			}
-			if (!agg->hc) {
-				uint64_t g0 = 0;
-				B200_TRY(agg_groups(agg, &g0));
-				uint64_t hint = 2 * (uint64_t)agg->path_groups_hc;
-				B200_TRY(b200_agg_hc_prepare(ctx, &agg->hc, L, agg->track_cnt, hint > 2 * g0 ? hint : 2 * g0));
-				// the groups the generic table already holds (the adaptation probe's rows) move into the new table: from
-				// here on every group lives there and finalize reads it directly
-				if (g0) {
-					B200_TRY(b200_agg_hc_absorb(ctx, agg->hc, L, agg->slots, agg->capacity, agg->track_cnt));
-					int grid = grid_for(agg->capacity * L.stride, 256, 4, ctx->sm_count * 8);
-					agg_init_kernel<<<grid, 256, 0, ctx->stream>>>(agg->slots, agg->capacity, L);
-					ctx->launches++;
-					CUDA_TRY(cudaMemsetAsync(agg->count, 0, 8, ctx->stream));
-					agg->counts_fresh = false;
-				}
-				agg->aos_empty = true;
-			}
+			// L2 for as long as the data allows.)  A table that cannot take the next chunk (it would pass its lifetime of
+			// rows, see b200_agg_hc_compatible, or nullable inputs appeared) is first merged into the generic table, and a
+			// new one takes the chunk.
 			uint64_t chunk = 1ULL << 20;
 			int quiet = 0; // consecutive chunks without a deferral or a growth
 			while (begin < n) {
 				uint64_t end = begin + chunk < n ? begin + chunk : n;
+				if (agg->hc && !b200_agg_hc_compatible(agg->hc, L, agg->track_cnt, end - begin)) {
+					B200_TRY(agg_flush_hc(agg));
+				}
+				if (!agg->hc) {
+					uint64_t g0 = 0;
+					B200_TRY(agg_groups(agg, &g0));
+					uint64_t hint = 2 * (uint64_t)agg->path_groups_hc;
+					B200_TRY(b200_agg_hc_prepare(ctx, &agg->hc, L, agg->track_cnt, hint > 2 * g0 ? hint : 2 * g0));
+					// the groups the generic table holds from the adaptation probe move into the new table: from here on
+					// every group lives there and finalize reads it directly.  Groups from a combine or an earlier table
+					// stay in the generic table (their sums may need all 128 bits), and finalize merges this table into it.
+					agg->aos_empty = g0 == 0;
+					if (g0 && b200_agg_hc_compatible(agg->hc, L, agg->track_cnt, agg->generic_rows)) {
+						B200_TRY(b200_agg_hc_absorb(ctx, agg->hc, L, agg->slots, agg->capacity, agg->track_cnt,
+						                            agg->generic_rows));
+						int grid = grid_for(agg->capacity * L.stride, 256, 4, ctx->sm_count * 8);
+						agg_init_kernel<<<grid, 256, 0, ctx->stream>>>(agg->slots, agg->capacity, L);
+						ctx->launches++;
+						CUDA_TRY(cudaMemsetAsync(agg->count, 0, 8, ctx->stream));
+						agg->counts_fresh = false;
+						agg->generic_rows = 0;
+						agg->aos_empty = true;
+					}
+				}
 				uint64_t cap_before = b200_agg_hc_capacity(agg->hc);
 				int rc = run_with_growth(
 				    agg, begin, end,
@@ -1031,6 +1042,7 @@ int b200_agg_sink(b200_agg *agg, const b200_batch *in, const int *key_cols, cons
 		if (rc != B200_OK) {
 			return rc;
 		}
+		agg->generic_rows = agg->generic_rows > ~0ULL - (end - begin) ? ~0ULL : agg->generic_rows + (end - begin);
 		if (path != PATH_GLOBAL && !agg->path_decided) {
 			// adaptation (the analogue of DecideAdaptation's HyperLogLog estimate): every row of the probe chunk has
 			// been aggregated - in shared memory or, on a miss, inline in the global table - so the table's group
@@ -1347,6 +1359,7 @@ int b200_agg_combine_states(b200_agg *agg, const b200_batch *states) {
 	CUDA_TRY(cudaSetDevice(ctx->device));
 	B200_TRY(agg_flush_hc(agg));
 	agg->counts_fresh = false;
+	agg->generic_rows = ~0ULL; // the states' sums may need all 128 bits
 	// exported states carry an explicit cnt(x) for every input: from now on cnt is tracked here as well
 	for (int i = 0; i < L.ninputs; i++) {
 		if (!agg->track_cnt[i]) {
@@ -1411,6 +1424,7 @@ int b200_agg_combine_packed(b200_agg *agg, const uint64_t *src_dev, int nranks, 
 	const AggLayout &L = agg->L;
 	CUDA_TRY(cudaSetDevice(ctx->device));
 	B200_TRY(agg_flush_hc(agg));
+	agg->generic_rows = ~0ULL; // the states' sums may need all 128 bits
 	// no deferral on this path: the table must have room for everything already in it plus every incoming group
 	uint64_t incoming = (uint64_t)nranks * max_groups;
 	if (agg->rows_seen != 0) {

@@ -735,7 +735,8 @@ __global__ void __launch_bounds__(256) agg_hc_flush_kernel(HcView H, uint64_t ca
 }
 
 // Move the groups of the generic table (the adaptation probe's rows) INTO this table, so that afterwards every group
-// lives here and finalize can read this table directly instead of merging it into the generic one.
+// lives here and finalize can read this table directly instead of merging it into the generic one.  A = bits 0..31 and
+// B = bits 32..95 of each 128-bit sum: exact only for sums of at most one table lifetime of rows (b200_agg_hc_absorb).
 template <int KW>
 __global__ void __launch_bounds__(256)
     agg_hc_absorb_kernel(HcView H, AggLayout L, const uint64_t *slots, uint64_t capacity, AggCols ac,
@@ -1015,14 +1016,18 @@ int b200_agg_hc_grow(b200_ctx *ctx, const AggLayout &L, AggHc *hc, uint64_t new_
 	return B200_OK;
 }
 
-// does the table `hc` still match the aggregate's state configuration (nullable inputs may have appeared)?
-bool b200_agg_hc_compatible(const AggHc *hc, const AggLayout &L, const bool *track_cnt) {
+// Can the table `hc` take `rows` more rows: does it still match the aggregate's state configuration (nullable inputs
+// may have appeared), and do the rows fit its lifetime?  Invariant: a group's A / B / rows words hold at most one table
+// lifetime of rows, at most 2^32, counted from zero (absorbed rows included), so that A (< 2^32 per row) and B (a
+// signed or unsigned high half per row) cannot wrap in their 64-bit words.  Everything beyond 96 bits stays in the
+// generic table's 128-bit sums: a table that is full is flushed into it and a new, empty one takes the next rows.
+bool b200_agg_hc_compatible(const AggHc *hc, const AggLayout &L, const bool *track_cnt, uint64_t rows) {
 	for (int i = 0; i < L.ninputs; i++) {
 		if (hc->track_cnt[i] != track_cnt[i]) {
 			return false;
 		}
 	}
-	return hc->rows_sunk < (1ULL << 31); // the 32-bit halves are summed in 64-bit words: merge before they could wrap
+	return rows <= (1ULL << 32) && hc->rows_sunk <= (1ULL << 32) - rows;
 }
 
 // Create the table (room for `groups_hint` groups at load <= 0.5) or grow an existing one to that size.
@@ -1258,9 +1263,12 @@ int b200_agg_hc_flush(b200_ctx *ctx, AggHc *hc, const AggLayout &L, const AggTab
 	return B200_OK;
 }
 
-// Empty the generic table's groups into this one (the caller re-initialises the generic table afterwards).
+// Empty the generic table's groups into this one (the caller re-initialises the generic table afterwards).  `rows`:
+// the rows the generic table's states hold; they count towards this table's lifetime, which must have room for them
+// (b200_agg_hc_compatible), so every 128-bit sum fits the 96 bits that A and B keep of it.
 int b200_agg_hc_absorb(b200_ctx *ctx, AggHc *hc, const AggLayout &L, const uint64_t *slots, uint64_t capacity,
-                       const bool *track_cnt) {
+                       const bool *track_cnt, uint64_t rows) {
+	hc->rows_sunk += rows;
 	AggCols ac;
 	memset(&ac, 0, sizeof(ac));
 	for (int i = 0; i < L.ninputs; i++) {
