@@ -122,6 +122,7 @@ def lib():
     L.b200_join_finalize.argtypes = [vp]
     L.b200_join_build_rows.argtypes = [vp, u64p]
     L.b200_join_probe.argtypes = [vp, vp, intp, intp, C.c_int, C.c_uint64, C.POINTER(vp), vp, u64p]
+    L.b200_join_probe_mark.argtypes = [vp, vp, intp, vp, vp]
     L.b200_join_destroy.argtypes = [vp]
     L.b200_join_destroy.restype = None
     L.b200_radix_partition.argtypes = [vp, vp, intp, C.c_int, C.c_int, C.POINTER(vp), u64p]
@@ -140,7 +141,7 @@ EXPORTED_SYMBOLS = [
     "b200_filter_project", "b200_agg_create", "b200_agg_sink", "b200_agg_group_count", "b200_agg_export_states",
     "b200_agg_combine_states", "b200_agg_packed_words", "b200_agg_export_packed", "b200_agg_combine_packed",
     "b200_agg_finalize", "b200_agg_destroy", "b200_join_create", "b200_join_build_sink",
-    "b200_join_finalize", "b200_join_build_rows", "b200_join_probe", "b200_join_destroy", "b200_radix_partition",
+    "b200_join_finalize", "b200_join_build_rows", "b200_join_probe", "b200_join_probe_mark", "b200_join_destroy", "b200_radix_partition",
     "b200_partition_count", "b200_partition_scatter", "b200_partition_count_dev", "b200_partition_scatter_dev",
 ]
 

@@ -20,6 +20,8 @@
 int b200_fill_keycols(const b200_batch *b, const int *cols, int n, KeyCols *out, const char *who);
 int b200_join_probe_tile(b200_ctx *ctx, const JoinView &J, const KeyCols &keys, const ProbeOut &po, int join_type,
                          uint64_t n, uint64_t out_capacity, unsigned long long *counters);
+int b200_join_probe_mark_launch(b200_ctx *ctx, const JoinView &J, const KeyCols &keys, uint64_t n, uint8_t *mark,
+                                uint64_t *validity);
 
 // ------------------------------------------------------------------ build
 __global__ void __launch_bounds__(256)
@@ -363,6 +365,43 @@ static int join_reserve(b200_join *j, uint64_t need_rows) {
 	return B200_OK;
 }
 
+// the probe key columns of a batch, checked against the types the join was created with
+static int probe_keycols(const b200_join *j, const b200_batch *probe, const int *key_cols, KeyCols *keys,
+                         const char *who) {
+	B200_TRY(b200_fill_keycols(probe, key_cols, j->nkeys, keys, who));
+	for (int k = 0; k < j->nkeys; k++) {
+		if (keys->c[k].type != j->key_type[k]) {
+			b200_set_error("%s: key %d has type %d, join was created with %d", who, k, keys->c[k].type, j->key_type[k]);
+			return B200_ERR_INVALID;
+		}
+	}
+	return B200_OK;
+}
+
+// what the probe kernels read of a finalized join
+static JoinView join_view(const b200_join *j) {
+	JoinView J;
+	memset(&J, 0, sizeof(J));
+	J.dense = j->dense;
+	J.dense_min = j->dense_min;
+	J.dense_range = j->dense_range;
+	J.slots = j->slots;
+	J.mask = j->table_cap - 1;
+	J.next = j->next;
+	J.exact = j->exact;
+	J.unique = j->unique;
+	J.inline_payload = j->inline_payload;
+	J.nkeys = j->nkeys;
+	for (int k = 0; k < j->nkeys; k++) {
+		J.key_type[k] = j->key_type[k];
+	}
+	J.ks = j->ks;
+	J.ps = j->ps;
+	J.build_has_null = j->has_null_key;
+	J.build_empty = j->rows == 0;
+	return J;
+}
+
 extern "C" {
 
 int b200_join_create(b200_ctx *ctx, int join_type, const int32_t *key_types, int nkeys, const int32_t *payload_types,
@@ -645,14 +684,7 @@ int b200_join_probe(b200_join *j, const b200_batch *probe, const int *key_cols, 
 	}
 	b200_ctx *ctx = j->ctx;
 	KeyCols keys;
-	B200_TRY(b200_fill_keycols(probe, key_cols, j->nkeys, &keys, "b200_join_probe"));
-	for (int k = 0; k < j->nkeys; k++) {
-		if (keys.c[k].type != j->key_type[k]) {
-			b200_set_error("b200_join_probe: key %d has type %d, join was created with %d", k, keys.c[k].type,
-			               j->key_type[k]);
-			return B200_ERR_INVALID;
-		}
-	}
+	B200_TRY(probe_keycols(j, probe, key_cols, &keys, "b200_join_probe"));
 	for (int i = 0; i < nlhs; i++) {
 		if (lhs_cols[i] < 0 || lhs_cols[i] >= (int)probe->cols.size()) {
 			b200_set_error("b200_join_probe: lhs column index %d out of range", lhs_cols[i]);
@@ -672,25 +704,7 @@ int b200_join_probe(b200_join *j, const b200_batch *probe, const int *key_cols, 
 	CUDA_TRY(cudaSetDevice(ctx->device));
 	*out = nullptr;
 	*out_count = 0;
-	JoinView J;
-	memset(&J, 0, sizeof(J));
-	J.dense = j->dense;
-	J.dense_min = j->dense_min;
-	J.dense_range = j->dense_range;
-	J.slots = j->slots;
-	J.mask = j->table_cap - 1;
-	J.next = j->next;
-	J.exact = j->exact;
-	J.unique = j->unique;
-	J.inline_payload = j->inline_payload;
-	J.nkeys = j->nkeys;
-	for (int k = 0; k < j->nkeys; k++) {
-		J.key_type[k] = j->key_type[k];
-	}
-	J.ks = j->ks;
-	J.ps = j->ps;
-	J.build_has_null = j->has_null_key;
-	J.build_empty = j->rows == 0;
+	JoinView J = join_view(j);
 	int jt = j->join_type;
 	bool with_payload = jt == B200_JOIN_INNER || jt == B200_JOIN_LEFT;
 	ProbeOut po;
@@ -787,6 +801,35 @@ int b200_join_probe(b200_join *j, const b200_batch *probe, const int *key_cols, 
 	*out = ob;
 	*out_count = count;
 	return B200_OK;
+}
+
+int b200_join_probe_mark(b200_join *j, const b200_batch *probe, const int *key_cols, uint8_t *mark_dev,
+                         uint64_t *mark_validity_dev) {
+	if (!j || !probe || !key_cols || !mark_dev || !mark_validity_dev) {
+		b200_set_error("b200_join_probe_mark: bad arguments");
+		return B200_ERR_INVALID;
+	}
+	// a join handle only exists where a context could be created; the check comes before the handle is read
+	if (b200_device_count() <= 0) {
+		b200_set_error("b200_join_probe_mark: no CUDA device available (there is no CPU fallback)");
+		return B200_ERR_NO_DEVICE;
+	}
+	if (j->join_type != B200_JOIN_MARK) {
+		b200_set_error("b200_join_probe_mark: the join was created as type %d, not B200_JOIN_MARK", j->join_type);
+		return B200_ERR_INVALID;
+	}
+	if (!j->finalized) {
+		b200_set_error("b200_join_probe_mark: call b200_join_finalize first");
+		return B200_ERR_INVALID;
+	}
+	KeyCols keys;
+	B200_TRY(probe_keycols(j, probe, key_cols, &keys, "b200_join_probe_mark"));
+	uint64_t n = probe->nrows;
+	if (n == 0) {
+		return B200_OK;
+	}
+	CUDA_TRY(cudaSetDevice(j->ctx->device));
+	return b200_join_probe_mark_launch(j->ctx, join_view(j), keys, n, mark_dev, mark_validity_dev);
 }
 
 } // extern "C"

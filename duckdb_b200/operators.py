@@ -405,6 +405,26 @@ class HashJoin:
                                     C.c_void_p(lhs_sel_dev) if lhs_sel_dev else None, C.byref(count)))
         return Batch(self.ctx, out), count.value
 
+    def probe_mark(self, batch, key_cols, mark_dev=None, validity_dev=None):
+        """MARK join in probe order (b200_join_probe_mark).  With caller-owned device buffers (mark_dev: nrows bytes,
+        validity_dev: (nrows + 63) // 64 uint64 words) the call only enqueues the kernel and returns None; without
+        them it allocates both, waits for the result and returns (mark uint8 ndarray, valid bool ndarray)."""
+        import torch  # device buffers for the result (plumbing only)
+
+        n = batch.nrows
+        own = mark_dev is None
+        if own:
+            mark_t = torch.empty(max(n, 1), dtype=torch.uint8, device=f"cuda:{self.ctx.device}")
+            valid_t = torch.empty(max((n + 63) // 64, 1), dtype=torch.int64, device=f"cuda:{self.ctx.device}")
+            mark_dev, validity_dev = mark_t.data_ptr(), valid_t.data_ptr()
+        check(lib().b200_join_probe_mark(self.handle, batch.handle, capi.int_array(key_cols), C.c_void_p(mark_dev),
+                                         C.c_void_p(validity_dev)))
+        if not own:
+            return None
+        self.ctx.sync()
+        words = valid_t[:(n + 63) // 64].cpu().numpy().view(np.uint64)
+        return mark_t[:n].cpu().numpy(), capi.valid_from_words(words, n)
+
     def close(self):
         if self.handle:
             lib().b200_join_destroy(self.handle)

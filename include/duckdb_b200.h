@@ -351,6 +351,26 @@ B200_API int b200_join_build_rows(b200_join *join, uint64_t *out_rows);
 B200_API int b200_join_probe(b200_join *join, const b200_batch *probe, const int *key_cols, const int *lhs_cols,
                              int nlhs, uint64_t out_capacity, b200_batch **out, uint32_t *out_lhs_sel,
                              uint64_t *out_count);
+/* Probe one batch of a finalized B200_JOIN_MARK join IN PROBE ORDER: for probe
+ * row i, mark_dev[i] (device, nrows bytes, BOOL 0 / 1) and bit i of
+ * mark_validity_dev (device, (nrows+63)/64 uint64 words, DuckDB validity_t
+ * words, bit = 1 valid; bits past row nrows-1 are unspecified):
+ *   TRUE  the probe key has a match;
+ *   NULL  the probe key is NULL, or it has no match and the build side holds a
+ *         NULL key;
+ *   FALSE otherwise, and for every row (NULL keys too) when the build side is
+ *         empty.
+ * Same key columns as b200_join_probe; no lhs columns are copied.  The call is
+ * stream-asynchronous: it enqueues one kernel on the context's stream and
+ * returns without synchronising.  B200_ERR_INVALID for a NULL argument, a join
+ * of another type or one not yet finalized; B200_ERR_NO_DEVICE without a CUDA
+ * device.  Replaces JoinHashTable::ConstructMarkJoinResult
+ * (join_hashtable.cpp:1978-2030) behind PhysicalHashJoin::ExecuteInternal
+ * (physical_hash_join.cpp:2140-2209) for MARK joins, and
+ * PhysicalComparisonJoin::ConstructEmptyJoinResult
+ * (physical_comparison_join.cpp:116-150) for an empty build side. */
+B200_API int b200_join_probe_mark(b200_join *join, const b200_batch *probe, const int *key_cols, uint8_t *mark_dev,
+                                  uint64_t *mark_validity_dev);
 B200_API void b200_join_destroy(b200_join *join);
 
 /* ---------------------------------------------------------- radix partition */

@@ -9,6 +9,11 @@
 // no residual predicate, build-side output columns of numeric physical types.  Probe-side output columns may have
 // ANY type: the kernel returns the probe row id of every result row and the operator slices the input chunk with
 // it (the same contract as ScanStructure::NextInnerJoin, join_hashtable.cpp:1737-1760).
+// MARK joins (large IN lists, IN subqueries that are not plain conjuncts) with ONE such condition, uncorrelated,
+// without build-side output columns: the result is every probe row plus a BOOL mark, in probe order
+// (b200_join_probe_mark), so each buffered input chunk is emitted whole with the mark vector appended.  Several
+// conditions are left to the stock operator, whose row-equality MARK join compares NULL components row by row
+// (JoinHashTable::InitializeUncorrelatedMarkJoin, physical_hash_join.cpp:710-720).
 // With a CUDA device: Sink batches build chunks into morsels -> b200_join_build_sink, Finalize ->
 // b200_join_finalize, Execute -> b200_join_probe per input chunk, results emitted in <= 2048-row slices
 // (HAVE_MORE_OUTPUT).  Without a device ("plumbing, no GPU") every call is forwarded to the wrapped operator.
@@ -34,13 +39,15 @@ static B200JoinPlan AnalyseJoin(const PhysicalHashJoin &op) {
 	case JoinType::LEFT:
 	case JoinType::SEMI:
 	case JoinType::ANTI:
+	case JoinType::MARK:
 		plan.join_type = static_cast<int32_t>(op.join_type); // b200_join_type uses duckdb::JoinType's values
 		break;
 	default:
 		return plan;
 	}
+	bool mark = op.join_type == JoinType::MARK;
 	if (op.predicate || op.residual_info || !op.delim_types.empty() || op.conditions.empty() ||
-	    op.conditions.size() > 8) {
+	    op.conditions.size() > (mark ? 1 : 8)) {
 		return plan;
 	}
 	for (auto &cond : op.conditions) {
@@ -81,7 +88,8 @@ static B200JoinPlan AnalyseJoin(const PhysicalHashJoin &op) {
 		return plan;
 	}
 	plan.lhs_output = op.lhs_output_columns.col_idxs;
-	if (op.types.size() != plan.lhs_output.size() + plan.payload.size()) {
+	if (op.types.size() != plan.lhs_output.size() + plan.payload.size() + (mark ? 1 : 0) ||
+	    (mark && op.types.back().id() != LogicalTypeId::BOOLEAN)) {
 		return plan;
 	}
 	plan.eligible = true;
@@ -133,16 +141,28 @@ public:
 	vector<vector<uint64_t>> payload_valid;
 	uint32_t *sel_dev = nullptr;               // device buffer for the probe row id of every result row
 	idx_t sel_capacity = 0;
+	// MARK join: one device block and its pinned host copy, [validity words | mark bytes] of the batch
+	void *mark_dev = nullptr;
+	uint8_t *mark_host = nullptr;
 
 	~B200JoinOperatorState() override {
 		if (sel_dev) {
 			cudaFree(sel_dev);
+		}
+		if (mark_dev) {
+			cudaFree(mark_dev);
+		}
+		if (mark_host) {
+			b200_host_free(nullptr, mark_host);
 		}
 	}
 	void Finalize(const PhysicalOperator &op, ExecutionContext &context) override;
 };
 
 static constexpr idx_t B200_PROBE_BATCH = 128 * 1024;
+//! MARK join block: validity words, then mark bytes, for a batch of at most one chunk past B200_PROBE_BATCH rows
+static constexpr idx_t B200_MARK_ROWS = B200_PROBE_BATCH + STANDARD_VECTOR_SIZE;
+static constexpr idx_t B200_MARK_VALID_BYTES = (B200_MARK_ROWS + 63) / 64 * 8;
 
 class B200JoinSourceState : public GlobalSourceState {
 public:
@@ -385,6 +405,10 @@ public:
 		for (idx_t k = 0; k < plan.probe_keys.size(); k++) {
 			key_cols.push_back(NumericCast<int>(k));
 		}
+		if (plan.join_type == B200_JOIN_MARK) {
+			ProbeMarkBatch(g, state, batch, key_cols);
+			return;
+		}
 		// result rows <= probe rows x longest duplicate chain; sized by the library (capacity 0) except for the row ids
 		b200_batch *out = nullptr;
 		uint64_t count = 0;
@@ -468,8 +492,81 @@ public:
 		}
 	}
 
+	//! MARK join: one in-order kernel call for the batch, then ONE copy of its marks and validity to the host
+	void ProbeMarkBatch(B200JoinGlobalState &g, B200JoinOperatorState &state, b200_batch *batch,
+	                    const vector<int> &key_cols) const {
+		int rc;
+		{
+			auto t_lock = make_uniq<B200Timer>(B200_T_LOCK_WAIT);
+			std::lock_guard<std::mutex> guard(g.lock); // one join object (one stream), driven from one thread at a time
+			t_lock.reset();
+			B200Timer timer(B200_T_KERNEL_CALL);
+			if (!state.mark_dev) {
+				if (cudaMalloc(&state.mark_dev, B200_MARK_VALID_BYTES + B200_MARK_ROWS) != cudaSuccess ||
+				    b200_host_alloc(g.ctx, B200_MARK_VALID_BYTES + B200_MARK_ROWS, reinterpret_cast<void **>(&state.mark_host)) != B200_OK) {
+					b200_batch_free(batch);
+					throw OutOfMemoryException("b200: cannot allocate the MARK join result buffers");
+				}
+			}
+			auto block = static_cast<uint8_t *>(state.mark_dev);
+			rc = b200_join_probe_mark(g.join, batch, key_cols.data(), block + B200_MARK_VALID_BYTES,
+			                          reinterpret_cast<uint64_t *>(block));
+			if (rc == B200_OK) {
+				rc = b200_ctx_sync(g.ctx);
+			}
+			b200_batch_free(batch);
+		}
+		B200Check(rc);
+		B200Timer timer(B200_T_DOWNLOAD);
+		if (cudaMemcpy(state.mark_host, state.mark_dev, B200_MARK_VALID_BYTES + state.buffered_rows,
+		               cudaMemcpyDeviceToHost) != cudaSuccess) {
+			throw IOException("b200: D2H of the MARK join result failed");
+		}
+	}
+
+	//! MARK join: the next buffered input chunk, whole, with its marks appended (ConstructMarkJoinResult's layout)
+	bool EmitNextMark(B200JoinOperatorState &state, DataChunk &chunk) const {
+		B200Timer timer(B200_T_EMIT);
+		if (state.emit_chunk >= state.buffered.size()) {
+			state.buffered.clear();
+			state.chunk_start.clear();
+			state.buffered_rows = 0;
+			state.draining = false;
+			chunk.SetCardinality(0);
+			return false;
+		}
+		idx_t c = state.emit_chunk++;
+		auto &src = *state.buffered[c];
+		idx_t count = src.size();
+		idx_t start = state.chunk_start[c];
+		idx_t nlhs = plan.lhs_output.size();
+		for (idx_t col = 0; col < nlhs; col++) {
+			chunk.data[col].Reference(src.data[plan.lhs_output[col]]);
+		}
+		auto &mark = chunk.data[nlhs];
+		mark.SetVectorType(VectorType::FLAT_VECTOR);
+		FlatVector::SetSize(mark, count_t(count));
+		chunk.SetChildCardinality(count); // after the references: a referenced constant vector is resized too
+		auto out = FlatVector::GetDataMutable<bool>(mark);
+		auto &mask = FlatVector::ValidityMutable(mark);
+		mask.SetAllValid(count);
+		auto valid = reinterpret_cast<const uint64_t *>(state.mark_host);
+		const uint8_t *marks = state.mark_host + B200_MARK_VALID_BYTES + start;
+		for (idx_t i = 0; i < count; i++) {
+			out[i] = marks[i] != 0;
+			idx_t row = start + i;
+			if (!((valid[row >> 6] >> (row & 63)) & 1)) {
+				mask.SetInvalid(i);
+			}
+		}
+		return true;
+	}
+
 	//! emit the next <= 2048 result rows; returns false when the batch is drained (buffers are released)
 	bool EmitNext(B200JoinOperatorState &state, DataChunk &chunk) const {
+		if (plan.join_type == B200_JOIN_MARK) {
+			return EmitNextMark(state, chunk);
+		}
 		B200Timer timer(B200_T_EMIT);
 		while (state.emit_chunk < state.buffered.size() &&
 		       state.chunk_results[state.emit_chunk] + state.emit_pos >= state.chunk_results[state.emit_chunk + 1]) {
