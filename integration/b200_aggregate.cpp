@@ -32,6 +32,7 @@ struct B200AggResult {
 	enum Kind { DIRECT, INT128_TO_RESULT, AVG_INT } kind;
 	int desc;       // index of the b200 aggregate (AVG_INT: the SUM, desc + 1 is the COUNT)
 	double scale;   // AVG over DECIMAL: 10^scale, else 1
+	bool int16;     // AVG_INT over an INT16 input (SMALLINT, DECIMAL(<=4)): divided in double, not long double
 };
 
 struct B200AggPlan {
@@ -63,7 +64,7 @@ static B200AggPlan AnalyseAggregate(const PhysicalHashAggregate &op) {
 			return plan;
 		}
 		auto name = aggr.Function().GetName().GetIdentifierName();
-		B200AggResult res {B200AggResult::DIRECT, NumericCast<int>(plan.descs.size()), 1.0};
+		B200AggResult res {B200AggResult::DIRECT, NumericCast<int>(plan.descs.size()), 1.0, false};
 		if (name == "count_star") {
 			plan.descs.push_back({B200_AGG_COUNT_STAR, B200_INT64, -1, 0});
 			plan.results.push_back(res);
@@ -109,16 +110,23 @@ static B200AggPlan AnalyseAggregate(const PhysicalHashAggregate &op) {
 		} else if (name == "min" || name == "max") {
 			plan.descs.push_back({name == "min" ? B200_AGG_MIN : B200_AGG_MAX, in_type, input, 0});
 		} else if (name == "avg") {
+			// only the AVGs that return a DOUBLE: over TIMESTAMP / TIME (and their _TZ forms) the result is of the input
+			// type, rounded by integer division (DiscreteAverageOperation, avg.cpp:127-144)
+			if (result_physical != PhysicalType::DOUBLE) {
+				return plan;
+			}
 			if (is_float) {
 				if (in_type != B200_DOUBLE) {
 					return plan;
 				}
 				plan.descs.push_back({B200_AGG_AVG, in_type, input, 0});
 			} else {
-				// IntegerAverageOperationHugeint::Finalize (avg.cpp:109-121): long double(sum) / (count * scale)
+				// INT16: IntegerAverageOperation::Finalize (avg.cpp:93-107), double(sum) / (double(count) * scale);
+				// INT32 / INT64: IntegerAverageOperationHugeint::Finalize (avg.cpp:109-121), the same in long double
 				plan.descs.push_back({B200_AGG_SUM, in_type, input, 0});
 				plan.descs.push_back({B200_AGG_COUNT, in_type, input, 0});
 				res.kind = B200AggResult::AVG_INT;
+				res.int16 = in_type == B200_INT16;
 				if (child->GetReturnType().id() == LogicalTypeId::DECIMAL) {
 					res.scale = std::pow(10.0, double(DecimalType::GetScale(child->GetReturnType())));
 				}
@@ -765,6 +773,10 @@ public:
 					auto cnt = reinterpret_cast<const int64_t *>(g.result_data[col + 1].data())[row];
 					if (cnt == 0) {
 						FlatVector::SetNull(vec, i, true);
+					} else if (res.int16) {
+						// one rounding, as the stock operator: dividing in long double first would round twice
+						FlatVector::GetDataMutableUnsafe<double>(vec)[i] =
+						    Hugeint::Cast<double>(sum) / (static_cast<double>(cnt) * res.scale);
 					} else {
 						long double divident = static_cast<long double>(cnt) * static_cast<long double>(res.scale);
 						FlatVector::GetDataMutableUnsafe<double>(vec)[i] =

@@ -131,7 +131,10 @@ def _plan(con, sql, env):
         return "\n".join(str(r[-1]) for r in con.fetchall("EXPLAIN " + sql))
 
 
-def _assert_same(got, exp, what):
+def _assert_same(got, exp, what, by_value=()):
+    """equal types, validity and values, floats bit for bit (any NaN equals any NaN).  Float columns named in
+    `by_value` compare by value (-0.0 equals 0.0): float group keys, which hold the first value a group saw, and MIN /
+    MAX over groups that hold both zeros"""
     assert [c.name for c in got] == [c.name for c in exp], what
     assert [(c.type_id, c.scale) for c in got] == [(c.type_id, c.scale) for c in exp], what
     for g, e in zip(got, exp):
@@ -144,7 +147,9 @@ def _assert_same(got, exp, what):
         a, b = g.values[ev], e.values[ev]
         if a.dtype.kind == "f":
             nan = np.isnan(b)
-            diff = (np.isnan(a) != nan) | (~nan & (a.view(np.uint64) != b.view(np.uint64)))
+            bits = np.dtype(f"u{a.dtype.itemsize}")    # FLOAT results are 4 bytes wide
+            same = (a == b) if g.name in by_value else (a.view(bits) == b.view(bits))
+            diff = (np.isnan(a) != nan) | (~nan & ~same)
         elif a.dtype == object:
             diff = np.array([x != y for x, y in zip(a, b)], dtype=bool)
         else:
@@ -153,9 +158,10 @@ def _assert_same(got, exp, what):
         assert bad.size == 0, (what, g.name, "values differ at", np.flatnonzero(ev)[bad[:10]], a[bad[:5]], b[bad[:5]])
 
 
-def _compare(con, settings, sql, env, planned, not_planned):
-    """in the child: the plan must name `planned` and not `not_planned`; then two decorated runs against one stock run.
-    -> (plan, the stock result without its HUGEINT / VARCHAR values, which are slow to pickle)"""
+def _compare(con, settings, sql, env, planned, not_planned, by_value=()):
+    """in the child: the plan must name `planned` and not `not_planned`; then two decorated runs against one stock run
+    (`by_value`: see _assert_same).  -> (plan, the stock result without its HUGEINT / VARCHAR values, which are slow to
+    pickle)"""
     for k, v in settings.items():
         con.execute(f"SET {k}='{v}'" if isinstance(v, str) else f"SET {k}={v}")
     plan = _plan(con, sql, env)
@@ -167,7 +173,7 @@ def _compare(con, settings, sql, env, planned, not_planned):
     with _Env(stock):
         exp = con.execute(sql)
     for i, g in enumerate(got):
-        _assert_same(g, exp, f"run {i + 1}: {sql}")
+        _assert_same(g, exp, f"run {i + 1}: {sql}", by_value)
     for c in exp:
         if c.values.dtype == object:
             c.values = None
