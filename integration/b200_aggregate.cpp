@@ -11,22 +11,17 @@
 // and calls b200_agg_sink; Finalize downloads [groups..., results...] and GetData emits them in <= 2048-row
 // chunks.  Without a device ("plumbing, no GPU") every call is forwarded to the wrapped stock operator.
 // Ineligible aggregates are not wrapped at all (the plan keeps the stock operator).
+#include "b200_binding.hpp"
+
 #include "duckdb/execution/operator/aggregate/physical_hash_aggregate.hpp"
 #include "duckdb/planner/expression/bound_aggregate_expression.hpp"
 #include "duckdb/planner/expression/bound_reference_expression.hpp"
 #include "duckdb/common/types/hugeint.hpp"
 #include "duckdb/common/vector/flat_vector.hpp"
-#include "duckdb/common/vector/unified_vector_format.hpp"
 
-#include <mutex>
+#include <cmath>
 
 namespace duckdb {
-
-struct B200Column {
-	idx_t chunk_col;       // column of the input DataChunk
-	int32_t type;          // b200_type
-	idx_t width;           // bytes
-};
 
 struct B200AggResult {
 	enum Kind { DIRECT, INT128_TO_RESULT, AVG_INT } kind;
@@ -151,356 +146,6 @@ static B200AggPlan AnalyseAggregate(const PhysicalHashAggregate &op) {
 	return plan;
 }
 
-//! a host-side morsel: flattened copies of the needed columns of many DataChunks
-struct B200Morsel {
-	vector<vector<data_t>> data;
-	vector<vector<uint8_t>> valid; // one byte per row (packed into validity words at flush time)
-	vector<bool> has_null;
-	idx_t rows = 0;
-
-	void Init(idx_t ncols) {
-		data.resize(ncols);
-		valid.resize(ncols);
-		has_null.assign(ncols, false);
-	}
-	//! flat b200_vector views of the buffered columns (validity words only for columns that saw a NULL)
-	void ToVectors(const vector<B200Column> &infos, vector<b200_vector> &cols, vector<vector<uint64_t>> &masks) {
-		idx_t ncols = data.size();
-		cols.resize(ncols);
-		masks.resize(ncols);
-		for (idx_t c = 0; c < ncols; c++) {
-			cols[c].type = infos[c].type;
-			cols[c].vector_type = B200_FLAT_VECTOR;
-			cols[c].data = data[c].data();
-			cols[c].sel = nullptr;
-			cols[c].validity = nullptr;
-			cols[c].dict_size = 0;
-			if (has_null[c]) {
-				masks[c].assign((rows + 63) / 64, 0);
-				for (idx_t i = 0; i < rows; i++) {
-					if (valid[c][i]) {
-						masks[c][i >> 6] |= uint64_t(1) << (i & 63);
-					}
-				}
-				cols[c].validity = masks[c].data();
-			}
-		}
-	}
-	void Clear() {
-		for (idx_t c = 0; c < data.size(); c++) {
-			data[c].clear();
-			valid[c].clear();
-			has_null[c] = false;
-		}
-		rows = 0;
-	}
-	//! append `count` rows of a DataChunk column (flat / constant / dictionary / sliced): values are gathered through
-	//! the selection of the unified format, NULL rows keep whatever bytes the vector holds and clear their flag
-	void Append(Vector &vec, idx_t col, idx_t count, idx_t width) {
-		UnifiedVectorFormat format;
-		vec.ToUnifiedFormat(format);
-		auto &d = data[col];
-		auto &v = valid[col];
-		idx_t old = d.size();
-		d.resize(old + count * width);
-		v.resize(rows + count, 1);
-		auto dst = d.data() + old;
-		if (!format.sel->IsSet()) {
-			memcpy(dst, format.data, count * width); // flat vector: rows are already consecutive
-		} else {
-			for (idx_t i = 0; i < count; i++) {
-				memcpy(dst + i * width, format.data + format.sel->get_index(i) * width, width);
-			}
-		}
-		if (format.validity.CanHaveNull()) {
-			for (idx_t i = 0; i < count; i++) {
-				if (!format.validity.RowIsValid(format.sel->get_index(i))) {
-					v[rows + i] = 0;
-					has_null[col] = true;
-				}
-			}
-		}
-	}
-};
-
-
-//! What one worker needs to stream morsels to the device: a context (= a CUDA stream), two pinned host buffers and two
-//! device buffers of the same size.  Creating these is expensive (stream + page-locking + cudaMalloc: ~5-10 ms per
-//! worker, 16 workers per operator, every query) and they are perfectly reusable, so released sets go to a process-wide
-//! pool and the next operator state picks one up - per query the row path then contains no allocation at all.
-struct B200StagingResources {
-	b200_ctx *ctx = nullptr;
-	data_ptr_t host[2] = {nullptr, nullptr};
-	data_ptr_t dev[2] = {nullptr, nullptr};
-	idx_t bytes = 0;
-
-	~B200StagingResources() {
-		for (int i = 0; i < 2; i++) {
-			if (dev[i]) {
-				cudaFree(dev[i]);
-			}
-			if (host[i]) {
-				b200_host_free(ctx, host[i]);
-			}
-		}
-		if (ctx) {
-			b200_ctx_destroy(ctx);
-		}
-	}
-};
-
-class B200StagingPool {
-public:
-	static unique_ptr<B200StagingResources> Acquire(int device, idx_t bytes) {
-		{
-			std::lock_guard<std::mutex> guard(Lock());
-			auto &pool = Pool();
-			idx_t best = pool.size();
-			for (idx_t i = 0; i < pool.size(); i++) {
-				if (pool[i]->bytes >= bytes && pool[i]->bytes <= 4 * bytes + (idx_t(1) << 20) &&
-				    (best == pool.size() || pool[i]->bytes < pool[best]->bytes)) {
-					best = i;
-				}
-			}
-			if (best != pool.size()) {
-				auto res = std::move(pool[best]);
-				pool.erase(pool.begin() + NumericCast<int64_t>(best));
-				return res;
-			}
-		}
-		auto res = make_uniq<B200StagingResources>();
-		{
-			B200Timer timer(B200_T_CTX);
-			B200Check(b200_ctx_create(device, nullptr, &res->ctx));
-		}
-		B200Timer timer(B200_T_STAGING_INIT);
-		res->bytes = bytes;
-		for (int i = 0; i < 2; i++) {
-			void *p = nullptr;
-			B200Check(b200_host_alloc(res->ctx, bytes, &p));
-			res->host[i] = data_ptr_cast(p);
-			void *d = nullptr;
-			if (cudaMalloc(&d, bytes) != cudaSuccess) {
-				throw OutOfMemoryException("b200: cannot allocate the device side of the morsel ring");
-			}
-			res->dev[i] = data_ptr_cast(d);
-		}
-		return res;
-	}
-	static void Release(unique_ptr<B200StagingResources> res) {
-		if (!res) {
-			return;
-		}
-		b200_ctx_sync(res->ctx); // nothing of the finished query is still in flight on this stream
-		std::lock_guard<std::mutex> guard(Lock());
-		if (Pool().size() < 96) {
-			Pool().push_back(std::move(res));
-		}
-	}
-
-private:
-	static std::mutex &Lock() {
-		static std::mutex lock;
-		return lock;
-	}
-	static vector<unique_ptr<B200StagingResources>> &Pool() {
-		static vector<unique_ptr<B200StagingResources>> pool;
-		return pool;
-	}
-};
-
-//! Contexts of the operators' global states (the aggregate / join object lives on it), pooled for the same reason
-class B200ContextPool {
-public:
-	static b200_ctx *Acquire(int device) {
-		{
-			std::lock_guard<std::mutex> guard(Lock());
-			if (!Pool().empty()) {
-				auto ctx = Pool().back();
-				Pool().pop_back();
-				return ctx;
-			}
-		}
-		B200Timer timer(B200_T_CTX);
-		b200_ctx *ctx = nullptr;
-		B200Check(b200_ctx_create(device, nullptr, &ctx));
-		return ctx;
-	}
-	static void Release(b200_ctx *ctx) {
-		if (!ctx) {
-			return;
-		}
-		b200_ctx_sync(ctx);
-		std::lock_guard<std::mutex> guard(Lock());
-		if (Pool().size() < 32) {
-			Pool().push_back(ctx);
-		} else {
-			b200_ctx_destroy(ctx);
-		}
-	}
-
-private:
-	static std::mutex &Lock() {
-		static std::mutex lock;
-		return lock;
-	}
-	static vector<b200_ctx *> &Pool() {
-		static vector<b200_ctx *> pool;
-		return pool;
-	}
-};
-
-//! Pinned, double-buffered staging of one worker thread's morsels (north_star: "DataChunk columns pinned and streamed to
-//! HBM in morsel-sized batches").  Chunks are appended column-wise into the ACTIVE pinned buffer; a full buffer is
-//! copied asynchronously into ITS device buffer on the worker's own context (= its own CUDA stream) while the following
-//! chunks fill the other pinned buffer; the operator consumes an uploaded batch one morsel later.  Workers therefore
-//! overlap their H2D copies with each other and with the kernels - the only serialised part is the (short, asynchronous)
-//! kernel launch itself.  Host and device rings are persistent (B200StagingPool): nothing is allocated per morsel.
-struct B200Staging {
-	struct Buffer {
-		data_ptr_t base = nullptr;     // pinned host buffer
-		data_ptr_t dev_base = nullptr; // its device twin
-		idx_t rows = 0;
-		vector<bool> has_null;
-		b200_batch *batch = nullptr; // upload in flight / done, not yet consumed
-	};
-	unique_ptr<B200StagingResources> res;
-	b200_ctx *ctx = nullptr;
-	Buffer buf[2];
-	int active = 0;
-	idx_t capacity = 0;
-	vector<B200Column> infos;
-	vector<idx_t> data_off, valid_off; // byte offsets inside a buffer
-	idx_t bytes = 0;
-
-	~B200Staging() {
-		for (auto &b : buf) {
-			if (b.batch) {
-				b200_batch_free(b.batch);
-			}
-		}
-		B200StagingPool::Release(std::move(res));
-	}
-
-	void Init(int device, const vector<B200Column> &infos_p, idx_t capacity_rows) {
-		infos = infos_p;
-		capacity = capacity_rows;
-		idx_t off = 0;
-		for (auto &c : infos) {
-			data_off.push_back(off);
-			off += (capacity * c.width + 255) & ~idx_t(255);
-		}
-		for (idx_t c = 0; c < infos.size(); c++) {
-			valid_off.push_back(off);
-			off += (((capacity + 63) / 64) * 8 + 255) & ~idx_t(255);
-		}
-		bytes = off;
-		res = B200StagingPool::Acquire(device, bytes);
-		ctx = res->ctx;
-		for (int i = 0; i < 2; i++) {
-			buf[i].base = res->host[i];
-			buf[i].dev_base = res->dev[i];
-			buf[i].has_null.assign(infos.size(), false);
-		}
-	}
-
-	idx_t Room() const {
-		return capacity - buf[active].rows;
-	}
-
-	//! append rows [from, from + count) of the chunk's columns `chunk_cols` (one per staged column)
-	void Append(DataChunk &chunk, idx_t from, idx_t count) {
-		B200Timer timer(B200_T_APPEND);
-		auto &b = buf[active];
-		for (idx_t c = 0; c < infos.size(); c++) {
-			auto &vec = chunk.data[infos[c].chunk_col];
-			idx_t width = infos[c].width;
-			UnifiedVectorFormat format;
-			vec.ToUnifiedFormat(format);
-			auto dst = b.base + data_off[c] + b.rows * width;
-			if (!format.sel->IsSet()) {
-				memcpy(dst, format.data + from * width, count * width); // flat vector: rows are already consecutive
-			} else {
-				for (idx_t i = 0; i < count; i++) {
-					memcpy(dst + i * width, format.data + format.sel->get_index(from + i) * width, width);
-				}
-			}
-			if (format.validity.CanHaveNull()) {
-				auto words = reinterpret_cast<uint64_t *>(b.base + valid_off[c]);
-				if (!b.has_null[c]) {
-					// first NULL-able vector of this morsel: every row so far is valid
-					for (idx_t w = 0; w < (b.rows + 63) / 64; w++) {
-						words[w] = ~uint64_t(0);
-					}
-					b.has_null[c] = true;
-				}
-				for (idx_t i = 0; i < count; i++) {
-					idx_t row = b.rows + i;
-					bool valid = format.validity.RowIsValid(format.sel->get_index(from + i));
-					uint64_t bit = uint64_t(1) << (row & 63);
-					if ((row & 63) == 0) {
-						words[row >> 6] = 0;
-					}
-					words[row >> 6] = valid ? (words[row >> 6] | bit) : (words[row >> 6] & ~bit);
-				}
-			} else if (b.has_null[c]) {
-				auto words = reinterpret_cast<uint64_t *>(b.base + valid_off[c]);
-				for (idx_t i = 0; i < count; i++) {
-					idx_t row = b.rows + i;
-					if ((row & 63) == 0) {
-						words[row >> 6] = 0;
-					}
-					words[row >> 6] |= uint64_t(1) << (row & 63);
-				}
-			}
-		}
-		b.rows += count;
-	}
-
-	//! the batch uploaded one morsel ago (its copy has completed), or nullptr
-	b200_batch *TakeUploaded() {
-		auto &other = buf[1 - active];
-		if (!other.batch) {
-			return nullptr;
-		}
-		{
-			B200Timer timer(B200_T_UPLOAD_WAIT);
-			B200Check(b200_ctx_sync(ctx)); // only that upload is on this stream
-		}
-		auto batch = other.batch;
-		other.batch = nullptr;
-		other.rows = 0;
-		other.has_null.assign(infos.size(), false);
-		return batch;
-	}
-
-	//! start the asynchronous upload of the active buffer and switch buffers (the other one must have been taken)
-	void SubmitActive() {
-		auto &b = buf[active];
-		if (b.rows == 0) {
-			return;
-		}
-		vector<b200_vector> cols(infos.size());
-		vector<void *> dev_data(infos.size()), dev_valid(infos.size());
-		for (idx_t c = 0; c < infos.size(); c++) {
-			cols[c].type = infos[c].type;
-			cols[c].vector_type = B200_FLAT_VECTOR;
-			cols[c].data = b.base + data_off[c];
-			cols[c].sel = nullptr;
-			cols[c].validity = b.has_null[c] ? reinterpret_cast<uint64_t *>(b.base + valid_off[c]) : nullptr;
-			cols[c].dict_size = 0;
-			dev_data[c] = b.dev_base + data_off[c];
-			dev_valid[c] = b.dev_base + valid_off[c];
-		}
-		{
-			B200Timer timer(B200_T_UPLOAD);
-			B200Check(b200_batch_upload_to(ctx, cols.data(), NumericCast<int>(cols.size()), b.rows, dev_data.data(),
-			                               dev_valid.data(), &b.batch));
-		}
-		active = 1 - active;
-	}
-};
-
 class B200AggGlobalState : public GlobalSinkState {
 public:
 	std::mutex lock;
@@ -520,28 +165,6 @@ public:
 		B200ContextPool::Release(ctx);
 	}
 };
-
-class B200AggLocalState : public LocalSinkState {
-public:
-	B200Staging staging;
-	unique_ptr<LocalSinkState> inner;
-};
-
-class B200AggSourceState : public GlobalSourceState {
-public:
-	idx_t position = 0;
-	unique_ptr<GlobalSourceState> inner;
-	idx_t MaxThreads() override {
-		return inner ? inner->MaxThreads() : 1;
-	}
-};
-
-class B200AggLocalSourceState : public LocalSourceState {
-public:
-	unique_ptr<LocalSourceState> inner;
-};
-
-static constexpr idx_t B200_MORSEL_ROWS = 1 << 20;
 
 class B200HashAggregate : public PhysicalOperator {
 public:
@@ -594,7 +217,7 @@ public:
 	}
 
 	unique_ptr<LocalSinkState> GetLocalSinkState(ExecutionContext &context) const override {
-		auto state = make_uniq<B200AggLocalState>();
+		auto state = make_uniq<B200LocalSinkState>();
 		if (!on_device) {
 			state->inner = inner.GetLocalSinkState(context);
 		} else {
@@ -629,36 +252,24 @@ public:
 	}
 
 	SinkResultType Sink(ExecutionContext &context, DataChunk &chunk, OperatorSinkInput &input) const override {
-		auto &l = input.local_state.Cast<B200AggLocalState>();
+		auto &l = input.local_state.Cast<B200LocalSinkState>();
 		if (!on_device) {
 			OperatorSinkInput inner_input {*inner.sink_state, *l.inner, input.interrupt_state};
 			return inner.Sink(context, chunk, inner_input);
 		}
 		auto &g = input.global_state.Cast<B200AggGlobalState>();
-		idx_t from = 0;
-		while (from < chunk.size()) {
-			idx_t count = MinValue<idx_t>(chunk.size() - from, l.staging.Room());
-			l.staging.Append(chunk, from, count);
-			from += count;
-			if (l.staging.Room() == 0) {
-				// the morsel uploaded while this one was being filled is consumed now; then this one starts its upload
-				SinkBatch(context, g, l.staging.TakeUploaded());
-				l.staging.SubmitActive();
-			}
-		}
+		l.staging.Feed(chunk, [&](b200_batch *batch) { SinkBatch(context, g, batch); });
 		return SinkResultType::NEED_MORE_INPUT;
 	}
 
 	SinkCombineResultType Combine(ExecutionContext &context, OperatorSinkCombineInput &input) const override {
-		auto &l = input.local_state.Cast<B200AggLocalState>();
+		auto &l = input.local_state.Cast<B200LocalSinkState>();
 		if (!on_device) {
 			OperatorSinkCombineInput inner_input {*inner.sink_state, *l.inner, input.interrupt_state};
 			return inner.Combine(context, inner_input);
 		}
 		auto &g = input.global_state.Cast<B200AggGlobalState>();
-		SinkBatch(context, g, l.staging.TakeUploaded());
-		l.staging.SubmitActive();
-		SinkBatch(context, g, l.staging.TakeUploaded());
+		l.staging.Drain([&](b200_batch *batch) { SinkBatch(context, g, batch); });
 		return SinkCombineResultType::FINISHED;
 	}
 
@@ -701,25 +312,25 @@ public:
 	}
 
 	unique_ptr<GlobalSourceState> GetGlobalSourceState(ClientContext &context) const override {
-		auto state = make_uniq<B200AggSourceState>();
+		auto state = make_uniq<B200SourceState>();
 		if (!on_device) {
 			state->inner = inner.GetGlobalSourceState(context);
 		}
 		return std::move(state);
 	}
 	unique_ptr<LocalSourceState> GetLocalSourceState(ExecutionContext &context, GlobalSourceState &gstate) const override {
-		auto state = make_uniq<B200AggLocalSourceState>();
+		auto state = make_uniq<B200LocalSourceState>();
 		if (!on_device) {
-			state->inner = inner.GetLocalSourceState(context, *gstate.Cast<B200AggSourceState>().inner);
+			state->inner = inner.GetLocalSourceState(context, *gstate.Cast<B200SourceState>().inner);
 		}
 		return std::move(state);
 	}
 
 	SourceResultType GetDataInternal(ExecutionContext &context, DataChunk &chunk,
 	                                 OperatorSourceInput &input) const override {
-		auto &src = input.global_state.Cast<B200AggSourceState>();
+		auto &src = input.global_state.Cast<B200SourceState>();
 		if (!on_device) {
-			OperatorSourceInput inner_input {*src.inner, *input.local_state.Cast<B200AggLocalSourceState>().inner,
+			OperatorSourceInput inner_input {*src.inner, *input.local_state.Cast<B200LocalSourceState>().inner,
 			                                 input.interrupt_state};
 			return inner.GetDataInternal(context, chunk, inner_input);
 		}

@@ -8,7 +8,6 @@
 #include "b200_filter.cpp"
 #include "b200_aggregate.cpp"
 #include "b200_join.cpp"
-#include "b200_filter_batched.cpp"
 
 #include "duckdb/execution/physical_plan_generator.hpp"
 #include "duckdb/execution/operator/projection/physical_projection.hpp"
@@ -47,13 +46,12 @@ struct LogicalB200Filter : public LogicalExtensionOperator {
 			fprintf(stderr, "[b200] LogicalB200Filter::CreatePlan\n");
 		}
 		auto &child = planner.CreatePlan(*children[0]);
-		// with a device: the streaming operator (one kernel call per 128 K buffered rows) when the whole predicate
-		// translates; B200Filter (PhysicalFilter's per-chunk contract, stock executor for what does not translate)
-		// otherwise, on the CPU box ("plumbing, no GPU") and with B200_FILTER_BATCH=0
+		// with a device: the streaming operator (one kernel call per B200_FILTER_BATCH buffered rows) when the whole
+		// predicate translates; B200Filter (PhysicalFilter run by the stock executor) otherwise and on the CPU box
+		// ("plumbing, no GPU")
 		auto predicate = ConjunctionOf(std::move(expressions));
-		const char *batch_env = getenv("B200_FILTER_BATCH");
 		optional_ptr<PhysicalOperator> made;
-		if (b200_device_count() > 0 && !(batch_env && atoll(batch_env) == 0)) {
+		if (b200_device_count() > 0) {
 			auto program = AnalyseFilter(*predicate, child.GetTypes());
 			if (program.eligible) {
 				made = planner.Make<B200BatchedFilter>(child.GetTypes(), std::move(predicate), std::move(program),

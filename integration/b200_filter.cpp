@@ -1,152 +1,31 @@
-// Reference-side binding (host C++, lives in DuckDB's tree as an in-tree extension source, see INTEGRATION.md):
-// a PhysicalOperator subclass that forwards DuckDB's PhysicalFilter work to libduckdb_b200.so through the C ABI.
+// Reference-side binding of the filter (host C++, see INTEGRATION.md).
 //
-//   class B200Filter : public PhysicalFilter            (src/include/duckdb/execution/operator/filter/physical_filter.hpp:19)
-//   replaces PhysicalFilter::ExecuteInternal             (src/execution/operator/filter/physical_filter.cpp:53-64)
+// B200BatchedFilter replaces PhysicalFilter::ExecuteInternal (src/execution/operator/filter/physical_filter.cpp:53-64)
+// when a device is present and the whole predicate translates.  It buffers input chunks (deep copies + the predicate's
+// columns in the worker's pinned staging ring) until B200_FILTER_BATCH rows (default 128 K) are there, evaluates the
+// predicate with ONE b200_filter_project call (out_sel = the surviving row ids, in input order) and emits the
+// survivors as slices of the buffered chunks (HAVE_MORE_OUTPUT, then FinalExecute for the tail) - the same shape as
+// the batched probe of B200HashJoin.  A CachingPhysicalOperator cannot batch (Execute / FinalExecute are final there),
+// hence a PhysicalOperator of its own.
 //
-// What it shows: (1) how a DataChunk column (UnifiedVectorFormat {sel,data,validity}) maps 1:1 onto b200_vector for
-// flat / constant / dictionary vectors, (2) how a bound expression tree maps onto b200_expr_node, (3) the error
-// convention (status code -> duckdb::Exception), (4) that the output is produced exactly like the stock operator
-// (chunk.Slice(input, sel, n) with the selection vector the kernel returned, or chunk.Reference(input)).
-// Unsupported expression shapes / types fall through to the base class = the stock CPU path for that operator.
+// What it shows: (1) how a bound expression tree maps onto b200_expr_node, (2) the error convention (status code ->
+// duckdb::Exception), (3) that the output is produced exactly like the stock operator (chunk.Slice(input, sel, n)
+// with the selection the kernel returned, or chunk.Reference(input)).
 //
-// This file is compile-checked against the reference headers by __graft_entry__.build() when /root/reference is
-// present (g++ -fsyntax-only); it is not linked into libduckdb_b200.so (the product has no DuckDB dependency).
-#include "duckdb/execution/operator/filter/physical_filter.hpp"
+// B200Filter is PhysicalFilter under the binding's name: it is planned without a device and for predicates that do
+// not translate, and every chunk takes the base class (the stock CPU path).
+#include "b200_binding.hpp"
+
 #include "duckdb/execution/expression_executor.hpp"
+#include "duckdb/execution/operator/filter/physical_filter.hpp"
+#include "duckdb/execution/physical_operator.hpp"
 #include "duckdb/planner/expression/bound_comparison_expression.hpp"
 #include "duckdb/planner/expression/bound_conjunction_expression.hpp"
 #include "duckdb/planner/expression/bound_constant_expression.hpp"
 #include "duckdb/planner/expression/bound_function_expression.hpp"
 #include "duckdb/planner/expression/bound_reference_expression.hpp"
-#include "duckdb/common/vector/unified_vector_format.hpp"
-#include "duckdb/common/exception.hpp"
-
-#include "duckdb_b200.h"
-
-#include <cuda_runtime_api.h>
-
-#include <atomic>
-#include <chrono>
 
 namespace duckdb {
-
-//! B200_TIMING=1: wall-clock nanoseconds per phase of the binding, summed over all worker threads and printed (and
-//! reset) by B200TimingReport() when an operator's global state is destroyed - where the time of a query goes between
-//! DuckDB's chunks and the kernels.
-enum B200Phase : int {
-	B200_T_CTX = 0, B200_T_STAGING_INIT, B200_T_APPEND, B200_T_COPY_CHUNK, B200_T_UPLOAD, B200_T_UPLOAD_WAIT, B200_T_LOCK_WAIT,
-	B200_T_KERNEL_CALL, B200_T_DOWNLOAD, B200_T_FINALIZE, B200_T_EMIT, B200_T_PHASES
-};
-static std::atomic<uint64_t> g_b200_ns[B200_T_PHASES];
-static std::atomic<uint64_t> g_b200_calls[B200_T_PHASES];
-static bool B200TimingOn() {
-	static const bool on = getenv("B200_TIMING") != nullptr;
-	return on;
-}
-struct B200Timer {
-	int phase;
-	std::chrono::steady_clock::time_point t0;
-	explicit B200Timer(int phase_p) : phase(phase_p) {
-		if (B200TimingOn()) {
-			t0 = std::chrono::steady_clock::now();
-		}
-	}
-	~B200Timer() {
-		if (B200TimingOn()) {
-			auto ns = std::chrono::duration_cast<std::chrono::nanoseconds>(std::chrono::steady_clock::now() - t0).count();
-			g_b200_ns[phase] += uint64_t(ns);
-			g_b200_calls[phase]++;
-		}
-	}
-};
-static void B200TimingReport(const char *what) {
-	if (!B200TimingOn()) {
-		return;
-	}
-	static const char *names[B200_T_PHASES] = {"ctx_create", "staging_init", "append", "copy_chunk", "upload_submit",
-	                                           "upload_wait", "lock_wait", "kernel_call", "download", "finalize", "emit"};
-	fprintf(stderr, "[b200 timing] %s:", what);
-	for (int i = 0; i < B200_T_PHASES; i++) {
-		uint64_t ns = g_b200_ns[i].exchange(0), calls = g_b200_calls[i].exchange(0);
-		if (calls) {
-			fprintf(stderr, " %s=%.2fms/%llu", names[i], double(ns) / 1e6, (unsigned long long)calls);
-		}
-	}
-	fprintf(stderr, "\n");
-}
-
-static void B200Check(int rc) {
-	if (rc == B200_OK) {
-		return;
-	}
-	// SURVEY.md 8b "Error convention": status codes become duckdb::Exception subclasses
-	if (rc == B200_ERR_OVERFLOW) {
-		throw OutOfRangeException(string(b200_last_error()));
-	}
-	if (rc == B200_ERR_OOM) {
-		throw OutOfMemoryException(string(b200_last_error()));
-	}
-	throw IOException("b200: " + string(b200_last_error()));
-}
-
-//! PhysicalType -> b200_type (identical numeric values by construction, include/duckdb_b200.h)
-static bool B200Type(PhysicalType t, int32_t &out) {
-	switch (t) {
-	case PhysicalType::BOOL:
-	case PhysicalType::UINT8:
-	case PhysicalType::INT8:
-	case PhysicalType::UINT16:
-	case PhysicalType::INT16:
-	case PhysicalType::UINT32:
-	case PhysicalType::INT32:
-	case PhysicalType::UINT64:
-	case PhysicalType::INT64:
-	case PhysicalType::FLOAT:
-	case PhysicalType::DOUBLE:
-		out = static_cast<int32_t>(t);
-		return true;
-	default:
-		return false; // VARCHAR, HUGEINT, nested: stock operator
-	}
-}
-
-//! One DataChunk column -> b200_vector.  `format` must outlive the upload.
-static bool ToB200Vector(Vector &vec, idx_t count, UnifiedVectorFormat &format, b200_vector &out) {
-	int32_t type;
-	if (!B200Type(vec.GetType().InternalType(), type)) {
-		return false;
-	}
-	out.type = type;
-	out.dict_size = 0;
-	switch (vec.GetVectorType()) {
-	case VectorType::FLAT_VECTOR:
-	case VectorType::CONSTANT_VECTOR:
-		vec.ToUnifiedFormat(format);
-		out.vector_type = vec.GetVectorType() == VectorType::FLAT_VECTOR ? B200_FLAT_VECTOR : B200_CONSTANT_VECTOR;
-		out.data = format.data;
-		out.sel = nullptr;
-		out.validity = format.validity.CanHaveNull() ? format.validity.GetData() : nullptr;
-		return true;
-	case VectorType::DICTIONARY_VECTOR: {
-		// value(i) = child[sel[i]]; validity is the CHILD's mask, indexed by dictionary position - exactly
-		// what ToUnifiedFormat returns (src/common/vector/dictionary_vector.cpp:65-76)
-		vec.ToUnifiedFormat(format);
-		auto dict_size = DictionaryVector::DictionarySize(vec);
-		if (!dict_size.IsValid()) {
-			return false; // unknown dictionary size: flatten on the stock path
-		}
-		out.vector_type = B200_DICTIONARY_VECTOR;
-		out.data = format.data;
-		out.sel = format.sel->data();
-		out.validity = format.validity.CanHaveNull() ? format.validity.GetData() : nullptr;
-		out.dict_size = dict_size.GetIndex();
-		return true;
-	}
-	default:
-		return false; // FSST / SEQUENCE / SHREDDED: stock operator
-	}
-}
 
 //! Bound expression tree -> b200_expr_node program (children before parents).  Returns the root or -1.
 static int TranslateExpression(const Expression &expr, vector<b200_expr_node> &prog) {
@@ -249,61 +128,63 @@ static int TranslateExpression(const Expression &expr, vector<b200_expr_node> &p
 	return NumericCast<int>(prog.size() - 1);
 }
 
-class B200FilterState : public CachingOperatorState {
-public:
-	explicit B200FilterState(ExecutionContext &context, const Expression &expr)
-	    : sel(STANDARD_VECTOR_SIZE), fallback(context.client, expr) {
-	}
-	~B200FilterState() override {
-		if (sel_dev) {
-			cudaFree(sel_dev);
-		}
-		if (ctx) {
-			b200_ctx_destroy(ctx);
-		}
-	}
-	b200_ctx *ctx = nullptr;    // one context (= one stream) per worker thread, like one local state per thread
-	uint32_t *sel_dev = nullptr; // STANDARD_VECTOR_SIZE selection indices on the device
-	SelectionVector sel;
-	ExpressionExecutor fallback; // stock path for chunks the GPU path cannot take
+
+static idx_t B200FilterBatchRows() {
+	// below one chunk (0 included) a batch is one chunk
+	const char *env = getenv("B200_FILTER_BATCH");
+	idx_t rows = env ? idx_t(atoll(env)) : idx_t(128) * 1024;
+	return rows < STANDARD_VECTOR_SIZE ? STANDARD_VECTOR_SIZE : rows;
+}
+
+//! The predicate as a kernel program over the staged columns; eligible only when every node translates
+struct B200FilterProgram {
+	bool eligible = false;
+	vector<b200_expr_node> nodes;
+	int root = -1;
+	vector<B200Column> columns; // input-chunk columns the program reads, in staging order
 };
 
-//! Drop-in for PhysicalFilter: same constructor, same types, same output contract.
+//! The kernel's expression program is bounded (B200_MAX_EXPR_NODES): a predicate that does not fit stays on the stock
+//! path instead of failing at run time.  Only the columns the predicate references are staged (pass-through columns
+//! of any type - VARCHAR, HUGEINT, nested - never leave the host: the output is a slice of the input).
+static B200FilterProgram AnalyseFilter(const Expression &expression, const vector<LogicalType> &input_types) {
+	B200FilterProgram plan;
+	plan.root = TranslateExpression(expression, plan.nodes);
+	if (plan.root < 0 || plan.nodes.size() > B200_MAX_EXPR_NODES) {
+		return plan;
+	}
+	for (auto &node : plan.nodes) {
+		if (node.op != B200_EXPR_COLREF) {
+			continue;
+		}
+		idx_t chunk_col = idx_t(node.col);
+		if (chunk_col >= input_types.size()) {
+			return plan;
+		}
+		idx_t pos = 0;
+		for (; pos < plan.columns.size() && plan.columns[pos].chunk_col != chunk_col; pos++) {
+		}
+		if (pos == plan.columns.size()) {
+			int32_t type;
+			auto physical = input_types[chunk_col].InternalType();
+			if (!B200Type(physical, type)) {
+				return plan;
+			}
+			plan.columns.push_back({chunk_col, type, GetTypeIdSize(physical)});
+		}
+		node.col = NumericCast<int32_t>(pos);
+	}
+	plan.eligible = !plan.columns.empty();
+	return plan;
+}
+
+//! Drop-in for PhysicalFilter: same constructor, same types, same output contract, every chunk on the stock path
 class B200Filter : public PhysicalFilter {
 public:
-	B200Filter(PhysicalPlan &physical_plan, vector<LogicalType> types, vector<unique_ptr<Expression>> select_list,
-	           idx_t estimated_cardinality)
-	    : PhysicalFilter(physical_plan, std::move(types), std::move(select_list), estimated_cardinality) {
-		// BASELINE config 1 ("plumbing, no GPU"): without a CUDA device the operator is planned all the same and
-		// every chunk takes the base-class (stock DuckDB) path; with a device the predicate runs in b200_filter_project
-		if (b200_device_count() > 0) {
-			root = TranslateExpression(*expression, program);
-			// the kernel's expression program is bounded (B200_MAX_EXPR_NODES): a predicate that does not fit stays on
-			// the stock path instead of failing at run time
-			if (root >= 0 && program.size() > B200_MAX_EXPR_NODES) {
-				root = -1;
-				program.clear();
-			}
-			// only the columns the predicate references are uploaded (pass-through columns of any type - VARCHAR,
-			// HUGEINT, nested - never leave the host: the output is a Slice of the input)
-			if (root >= 0) {
-				for (auto &node : program) {
-					if (node.op == B200_EXPR_COLREF) {
-						idx_t pos = 0;
-						for (; pos < used_columns.size() && used_columns[pos] != idx_t(node.col); pos++) {
-						}
-						if (pos == used_columns.size()) {
-							used_columns.push_back(idx_t(node.col));
-						}
-						node.col = NumericCast<int32_t>(pos);
-					}
-				}
-			}
-		}
-	}
+	using PhysicalFilter::PhysicalFilter;
 
 	string GetName() const override {
-		return root >= 0 ? "B200_FILTER" : "B200_FILTER(host)";
+		return "B200_FILTER(host)";
 	}
 
 	//! EXPLAIN shows which path the operator takes
@@ -312,70 +193,145 @@ public:
 		result["Operator"] = GetName();
 		return result;
 	}
+};
+
+class B200BatchedFilterState : public B200BatchState {
+public:
+	B200BatchedFilterState(ExecutionContext &context, const Expression &expr) : fallback(context.client, expr) {
+	}
+	~B200BatchedFilterState() override {
+		if (report) {
+			B200TimingReport("filter (one worker's state; phases are summed over all workers since the last report)");
+		}
+	}
+	vector<uint32_t> row_ids;               // surviving batch rows, ascending
+	idx_t survivors = 0;
+	ExpressionExecutor fallback;            // stock path for a batch the kernel refuses (B200_ERR_INVALID)
+	bool report = true;
+};
+
+class B200BatchedFilter : public PhysicalOperator {
+public:
+	B200BatchedFilter(PhysicalPlan &physical_plan, vector<LogicalType> types, unique_ptr<Expression> expression_p,
+	                  B200FilterProgram program_p, idx_t estimated_cardinality)
+	    : PhysicalOperator(physical_plan, PhysicalOperatorType::EXTENSION, std::move(types), estimated_cardinality),
+	      expression(std::move(expression_p)), program(std::move(program_p)), batch_rows(B200FilterBatchRows()) {
+	}
+
+	unique_ptr<Expression> expression;
+	B200FilterProgram program;
+	idx_t batch_rows;
+
+	string GetName() const override {
+		return "B200_FILTER";
+	}
+	InsertionOrderPreservingMap<string> ParamsToString() const override {
+		InsertionOrderPreservingMap<string> result;
+		result["Operator"] = "B200_FILTER (batched, " + to_string(batch_rows) + " rows per kernel call)";
+		result["Expression"] = expression->ToString();
+		return result;
+	}
+	bool ParallelOperator() const override {
+		return true;
+	}
+	bool RequiresFinalExecute() const override {
+		return true; // the last, partial batch is evaluated at the end
+	}
 
 	unique_ptr<OperatorState> GetOperatorState(ExecutionContext &context) const override {
-		auto state = make_uniq<B200FilterState>(context, *expression);
-		if (root >= 0) {
-			B200Check(b200_ctx_create(0, nullptr, &state->ctx));
-			if (cudaMalloc(reinterpret_cast<void **>(&state->sel_dev), STANDARD_VECTOR_SIZE * sizeof(uint32_t)) !=
-			    cudaSuccess) {
-				throw OutOfMemoryException("b200: cannot allocate the selection buffer");
-			}
-		}
+		auto state = make_uniq<B200BatchedFilterState>(context, *expression);
+		state->staging.Init(0, program.columns, batch_rows + STANDARD_VECTOR_SIZE);
 		return std::move(state);
 	}
 
-protected:
-	OperatorResultType ExecuteInternal(ExecutionContext &context, DataChunk &input, DataChunk &chunk,
-	                                   GlobalOperatorState &gstate, OperatorState &state_p) const override {
-		auto &state = state_p.Cast<B200FilterState>();
-		idx_t result_count = 0;
-		bool done = false;
-		if (root >= 0) {
-			// DataChunk -> b200 batch of the columns the predicate reads
-			vector<UnifiedVectorFormat> formats(used_columns.size());
-			vector<b200_vector> cols(used_columns.size());
-			bool ok = true;
-			for (idx_t c = 0; c < used_columns.size() && ok; c++) {
-				ok = ToB200Vector(input.data[used_columns[c]], input.size(), formats[c], cols[c]);
-			}
-			if (ok) {
-				b200_batch *batch = nullptr;
-				B200Check(b200_batch_upload(state.ctx, cols.data(), NumericCast<int>(cols.size()), input.size(), &batch));
-				uint64_t count = 0;
-				int rc = b200_filter_project(state.ctx, batch, program.data(), NumericCast<int>(program.size()), root,
-				                             nullptr, 0, nullptr, state.sel_dev, nullptr, &count);
-				b200_batch_free(batch);
-				if (rc != B200_ERR_INVALID) {
-					B200Check(rc); // CUDA errors, out of memory, arithmetic overflow are real errors
-					if (count > 0 && count < input.size()) {
-						// true_sel of BinaryExecutor::Select, produced on the device
-						if (cudaMemcpy(state.sel.data(), state.sel_dev, count * sizeof(sel_t), cudaMemcpyDeviceToHost) !=
-						    cudaSuccess) {
-							throw IOException("b200: D2H of the selection vector failed");
-						}
-					}
-					result_count = count;
-					done = true;
+	//! ONE kernel call for everything buffered; row_ids = the survivors in input order
+	void FilterBatch(B200BatchedFilterState &state, b200_batch *batch) const {
+		idx_t n = state.buffered_rows;
+		state.survivors = 0;
+		state.ReserveSel(n, batch);
+		uint64_t count = 0;
+		B200Timer timer(B200_T_KERNEL_CALL);
+		int rc = b200_filter_project(state.staging.ctx, batch, program.nodes.data(), NumericCast<int>(program.nodes.size()),
+		                             program.root, nullptr, 0, nullptr, state.sel_dev, nullptr, &count);
+		b200_batch_free(batch);
+		state.row_ids.resize(n + 1);
+		if (rc == B200_ERR_INVALID) {
+			// a shape the kernel does not take: the stock executor selects chunk by chunk
+			SelectionVector sel(STANDARD_VECTOR_SIZE);
+			idx_t out = 0;
+			for (idx_t c = 0; c < state.buffered.size(); c++) {
+				idx_t k = state.fallback.SelectExpression(*state.buffered[c], sel);
+				for (idx_t i = 0; i < k; i++) {
+					state.row_ids[out++] = NumericCast<uint32_t>(state.chunk_start[c] + sel.get_index(i));
 				}
-				// B200_ERR_INVALID: a shape the kernel does not take - the stock executor handles this chunk
 			}
+			state.survivors = out;
+			return;
 		}
-		if (!done) {
-			result_count = state.fallback.SelectExpression(input, state.sel); // stock CPU path for this chunk
+		B200Check(rc);
+		if (count > 0 &&
+		    cudaMemcpy(state.row_ids.data(), state.sel_dev, count * sizeof(uint32_t), cudaMemcpyDeviceToHost) != cudaSuccess) {
+			throw IOException("b200: D2H of the selection vector failed");
 		}
-		if (result_count == input.size()) {
-			chunk.Reference(input); // nothing was filtered (physical_filter.cpp:57-59)
-		} else if (result_count > 0) {
-			chunk.Slice(input, state.sel, result_count); // dictionary vectors over the input, zero copy (:60-61)
-		}
-		return OperatorResultType::NEED_MORE_INPUT;
+		state.survivors = count;
 	}
 
-private:
-	vector<b200_expr_node> program;
-	vector<idx_t> used_columns; // input columns the program references, in program order
-	int root = -1;
+	//! emit the survivors of the next buffered chunk that has any; false when the batch is drained
+	bool EmitNext(B200BatchedFilterState &state, DataChunk &chunk) const {
+		B200Timer timer(B200_T_EMIT);
+		while (state.emit_chunk < state.buffered.size()) {
+			idx_t c = state.emit_chunk++;
+			auto &src = *state.buffered[c];
+			idx_t begin = state.chunk_start[c], end = begin + src.size();
+			idx_t first = state.emit_pos;
+			while (state.emit_pos < state.survivors && state.row_ids[state.emit_pos] < end) {
+				state.emit_pos++;
+			}
+			idx_t count = state.emit_pos - first;
+			if (count == 0) {
+				continue;
+			}
+			if (count == src.size()) {
+				chunk.Reference(src); // nothing was filtered (physical_filter.cpp:57-59)
+			} else {
+				SelectionVector sel(STANDARD_VECTOR_SIZE);
+				for (idx_t i = 0; i < count; i++) {
+					sel.set_index(i, state.row_ids[first + i] - begin);
+				}
+				chunk.Slice(src, sel, count); // dictionary vectors over the buffered chunk, zero copy (:60-61)
+			}
+			return true;
+		}
+		return false;
+	}
+
+	OperatorResultType Execute(ExecutionContext &context, DataChunk &input, DataChunk &chunk, GlobalOperatorState &gstate,
+	                           OperatorState &state_p) const override {
+		auto &state = state_p.Cast<B200BatchedFilterState>();
+		return state.Execute(
+		    context, input, chunk, batch_rows, [&](b200_batch *batch) { FilterBatch(state, batch); },
+		    [&](DataChunk &out) { return EmitNext(state, out); });
+	}
+
+	OperatorFinalizeResultType FinalExecute(ExecutionContext &context, DataChunk &chunk, GlobalOperatorState &gstate,
+	                                        OperatorState &state_p) const override {
+		auto &state = state_p.Cast<B200BatchedFilterState>();
+		return state.FinalExecute(
+		    context, chunk, [&](b200_batch *batch) { FilterBatch(state, batch); },
+		    [&](DataChunk &out) { return EmitNext(state, out); });
+	}
 };
+
+//! the select list of a LogicalFilter as ONE expression (PhysicalFilter's constructor, physical_filter.cpp:10-21)
+static unique_ptr<Expression> ConjunctionOf(vector<unique_ptr<Expression>> select_list) {
+	if (select_list.size() == 1) {
+		return std::move(select_list[0]);
+	}
+	auto conjunction = make_uniq<BoundConjunctionExpression>(ExpressionType::CONJUNCTION_AND);
+	for (auto &expr : select_list) {
+		conjunction->GetChildrenMutable().push_back(std::move(expr));
+	}
+	return std::move(conjunction);
+}
 
 } // namespace duckdb

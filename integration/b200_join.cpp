@@ -1,4 +1,3 @@
-#include <algorithm>
 // Reference-side binding of the hash join (see INTEGRATION.md): B200HashJoin, a sink (build side) + operator
 // (probe side) that DECORATES the stock PhysicalHashJoin the reference's planner produced.
 //
@@ -14,12 +13,19 @@
 // (b200_join_probe_mark), so each buffered input chunk is emitted whole with the mark vector appended.  Several
 // conditions are left to the stock operator, whose row-equality MARK join compares NULL components row by row
 // (JoinHashTable::InitializeUncorrelatedMarkJoin, physical_hash_join.cpp:710-720).
-// With a CUDA device: Sink batches build chunks into morsels -> b200_join_build_sink, Finalize ->
-// b200_join_finalize, Execute -> b200_join_probe per input chunk, results emitted in <= 2048-row slices
-// (HAVE_MORE_OUTPUT).  Without a device ("plumbing, no GPU") every call is forwarded to the wrapped operator.
+// With a CUDA device: Sink streams build chunks through the worker's staging ring -> b200_join_build_sink per
+// morsel, Finalize -> b200_join_finalize, Execute -> b200_join_probe per batch of buffered input chunks, results
+// emitted in <= 2048-row slices (HAVE_MORE_OUTPUT).  Without a device ("plumbing, no GPU") every call is forwarded to
+// the wrapped operator.
+#include "b200_binding.hpp"
+
+#include "duckdb/common/vector/flat_vector.hpp"
 #include "duckdb/execution/operator/join/physical_hash_join.hpp"
 #include "duckdb/parallel/meta_pipeline.hpp"
 #include "duckdb/parallel/pipeline.hpp"
+#include "duckdb/planner/expression/bound_reference_expression.hpp"
+
+#include <algorithm>
 
 namespace duckdb {
 
@@ -111,44 +117,23 @@ public:
 	}
 };
 
-class B200JoinLocalState : public LocalSinkState {
-public:
-	B200Morsel morsel;
-	unique_ptr<LocalSinkState> inner;
-};
-
-//! Probe-side state of one worker: input chunks are buffered (deep copies + their key columns in a pinned staging
-//! buffer) until a batch of B200_PROBE_BATCH rows is full, ONE b200_join_probe call handles the batch, and the result
-//! rows are emitted chunk by chunk (HAVE_MORE_OUTPUT, then FinalExecute for the tail).  A per-chunk probe would be
-//! one synchronous H2D -> kernel -> D2H round trip per 2048 rows.
-class B200JoinOperatorState : public OperatorState {
+//! Probe-side state of one worker: batches of B200_PROBE_BATCH rows (their key columns staged), ONE b200_join_probe
+//! call per batch
+class B200JoinOperatorState : public B200BatchState {
 public:
 	unique_ptr<OperatorState> inner; // host mode
-	// device mode
-	B200Staging staging;                       // key columns of the buffered rows (pinned, uploaded on this worker's stream)
-	vector<unique_ptr<DataChunk>> buffered;    // copies of the buffered input chunks (their vectors back the output slices)
-	vector<idx_t> chunk_start;                 // first batch row of every buffered chunk
-	idx_t buffered_rows = 0;
-	bool input_taken = false;                  // the current input chunk is already in the buffer
 	// results of the last probed batch, grouped by input chunk
-	bool draining = false;
 	vector<uint32_t> row_ids;                  // batch row of every result row, as returned
 	vector<uint32_t> row_chunk;                // buffered chunk of every batch row
 	vector<uint32_t> order;                    // result rows ordered by input chunk
 	vector<idx_t> chunk_results;               // prefix: results of chunk c are order[chunk_results[c] .. chunk_results[c+1])
-	idx_t emit_chunk = 0, emit_pos = 0;
 	vector<vector<data_t>> payload_data;
 	vector<vector<uint64_t>> payload_valid;
-	uint32_t *sel_dev = nullptr;               // device buffer for the probe row id of every result row
-	idx_t sel_capacity = 0;
 	// MARK join: one device block and its pinned host copy, [validity words | mark bytes] of the batch
 	void *mark_dev = nullptr;
 	uint8_t *mark_host = nullptr;
 
 	~B200JoinOperatorState() override {
-		if (sel_dev) {
-			cudaFree(sel_dev);
-		}
 		if (mark_dev) {
 			cudaFree(mark_dev);
 		}
@@ -163,19 +148,6 @@ static constexpr idx_t B200_PROBE_BATCH = 128 * 1024;
 //! MARK join block: validity words, then mark bytes, for a batch of at most one chunk past B200_PROBE_BATCH rows
 static constexpr idx_t B200_MARK_ROWS = B200_PROBE_BATCH + STANDARD_VECTOR_SIZE;
 static constexpr idx_t B200_MARK_VALID_BYTES = (B200_MARK_ROWS + 63) / 64 * 8;
-
-class B200JoinSourceState : public GlobalSourceState {
-public:
-	unique_ptr<GlobalSourceState> inner;
-	idx_t MaxThreads() override {
-		return inner ? inner->MaxThreads() : 1;
-	}
-};
-
-class B200JoinLocalSourceState : public LocalSourceState {
-public:
-	unique_ptr<LocalSourceState> inner;
-};
 
 class B200HashJoin : public PhysicalOperator {
 public:
@@ -268,68 +240,61 @@ public:
 	}
 
 	unique_ptr<LocalSinkState> GetLocalSinkState(ExecutionContext &context) const override {
-		auto state = make_uniq<B200JoinLocalState>();
+		auto state = make_uniq<B200LocalSinkState>();
 		if (!on_device) {
 			state->inner = inner.GetLocalSinkState(context);
 		} else {
-			state->morsel.Init(plan.build_keys.size() + plan.payload.size());
+			vector<B200Column> infos = plan.build_keys;
+			infos.insert(infos.end(), plan.payload.begin(), plan.payload.end());
+			state->staging.Init(0, infos, B200_MORSEL_ROWS);
 		}
 		return std::move(state);
 	}
 
-	void FlushBuild(B200JoinGlobalState &g, B200Morsel &m) const {
-		if (m.rows == 0) {
+	//! sink one uploaded morsel of build rows: the join object lives on the global context and is driven by one thread
+	//! at a time
+	void SinkBuildBatch(B200JoinGlobalState &g, b200_batch *batch) const {
+		if (!batch) {
 			return;
 		}
-		vector<B200Column> infos = plan.build_keys;
-		infos.insert(infos.end(), plan.payload.begin(), plan.payload.end());
-		vector<b200_vector> cols;
-		vector<vector<uint64_t>> masks;
-		m.ToVectors(infos, cols, masks);
 		vector<int> key_cols, payload_cols;
-		for (idx_t c = 0; c < infos.size(); c++) {
+		for (idx_t c = 0; c < plan.build_keys.size() + plan.payload.size(); c++) {
 			(c < plan.build_keys.size() ? key_cols : payload_cols).push_back(NumericCast<int>(c));
 		}
+		int rc;
 		{
+			auto t_lock = make_uniq<B200Timer>(B200_T_LOCK_WAIT);
 			std::lock_guard<std::mutex> guard(g.lock);
-			B200Timer timer(B200_T_FINALIZE); // build side: upload + b200_join_build_sink
-			b200_batch *batch = nullptr;
-			B200Check(b200_batch_upload(g.ctx, cols.data(), NumericCast<int>(cols.size()), m.rows, &batch));
-			int rc = b200_join_build_sink(g.join, batch, key_cols.data(), payload_cols.empty() ? nullptr : payload_cols.data());
+			t_lock.reset();
+			B200Timer timer(B200_T_KERNEL_CALL);
+			rc = b200_join_build_sink(g.join, batch, key_cols.data(), payload_cols.empty() ? nullptr : payload_cols.data());
+			// the build kernels read the worker's ring buffer asynchronously on the join's stream, and the ring refills
+			// that buffer two morsels later
 			b200_ctx_sync(g.ctx);
-			b200_batch_free(batch);
-			B200Check(rc);
 		}
-		m.Clear();
+		b200_batch_free(batch);
+		B200Check(rc);
 	}
 
 	SinkResultType Sink(ExecutionContext &context, DataChunk &chunk, OperatorSinkInput &input) const override {
-		auto &l = input.local_state.Cast<B200JoinLocalState>();
+		auto &l = input.local_state.Cast<B200LocalSinkState>();
 		if (!on_device) {
 			OperatorSinkInput inner_input {*inner.sink_state, *l.inner, input.interrupt_state};
 			return inner.Sink(context, chunk, inner_input);
 		}
-		idx_t c = 0;
-		for (auto &k : plan.build_keys) {
-			l.morsel.Append(chunk.data[k.chunk_col], c++, chunk.size(), k.width);
-		}
-		for (auto &p : plan.payload) {
-			l.morsel.Append(chunk.data[p.chunk_col], c++, chunk.size(), p.width);
-		}
-		l.morsel.rows += chunk.size();
-		if (l.morsel.rows >= B200_MORSEL_ROWS) {
-			FlushBuild(input.global_state.Cast<B200JoinGlobalState>(), l.morsel);
-		}
+		auto &g = input.global_state.Cast<B200JoinGlobalState>();
+		l.staging.Feed(chunk, [&](b200_batch *batch) { SinkBuildBatch(g, batch); });
 		return SinkResultType::NEED_MORE_INPUT;
 	}
 
 	SinkCombineResultType Combine(ExecutionContext &context, OperatorSinkCombineInput &input) const override {
-		auto &l = input.local_state.Cast<B200JoinLocalState>();
+		auto &l = input.local_state.Cast<B200LocalSinkState>();
 		if (!on_device) {
 			OperatorSinkCombineInput inner_input {*inner.sink_state, *l.inner, input.interrupt_state};
 			return inner.Combine(context, inner_input);
 		}
-		FlushBuild(input.global_state.Cast<B200JoinGlobalState>(), l.morsel);
+		auto &g = input.global_state.Cast<B200JoinGlobalState>();
+		l.staging.Drain([&](b200_batch *batch) { SinkBuildBatch(g, batch); });
 		return SinkCombineResultType::FINISHED;
 	}
 
@@ -370,37 +335,11 @@ public:
 		return std::move(state);
 	}
 
-	//! keep a copy of the input chunk and stage its key columns
-	void BufferInput(ExecutionContext &context, B200JoinOperatorState &state, DataChunk &input) const {
-		if (input.size() == 0) {
-			return;
-		}
-		auto copy = make_uniq<DataChunk>();
-		{
-			B200Timer timer(B200_T_COPY_CHUNK);
-			copy->Initialize(Allocator::Get(context.client), input.GetTypes());
-			input.Copy(*copy);
-		}
-		state.staging.Append(*copy, 0, copy->size());
-		state.chunk_start.push_back(state.buffered_rows);
-		state.buffered_rows += copy->size();
-		state.buffered.push_back(std::move(copy));
-	}
-
 	//! probe everything buffered with ONE kernel call; group the result rows by input chunk
-	void ProbeBatch(ExecutionContext &context, B200JoinGlobalState &g, B200JoinOperatorState &state) const {
-		context.client.InterruptCheck();
-		state.draining = true;
-		state.emit_chunk = 0;
-		state.emit_pos = 0;
+	void ProbeBatch(B200JoinGlobalState &g, B200JoinOperatorState &state, b200_batch *batch) const {
 		idx_t n = state.buffered_rows;
 		state.chunk_results.assign(state.buffered.size() + 1, 0);
 		state.order.clear();
-		if (n == 0) {
-			return;
-		}
-		state.staging.SubmitActive();                   // H2D of the key columns on this worker's stream
-		b200_batch *batch = state.staging.TakeUploaded(); // ... and wait for it (only this worker blocks)
 		vector<int> key_cols;
 		for (idx_t k = 0; k < plan.probe_keys.size(); k++) {
 			key_cols.push_back(NumericCast<int>(k));
@@ -420,31 +359,14 @@ public:
 			B200Timer timer(B200_T_KERNEL_CALL);
 			// one pass when the result fits n rows (always, for a unique build key: PK-FK joins); duplicates on the build
 			// side can produce more rows than probes: then a counting call sizes the second attempt exactly
-			auto ensure_sel = [&](uint64_t rows) {
-				if (state.sel_capacity >= rows) {
-					return true;
-				}
-				if (state.sel_dev) {
-					cudaFree(state.sel_dev);
-					state.sel_dev = nullptr;
-				}
-				state.sel_capacity = rows + rows / 4 + 1024;
-				return cudaMalloc(reinterpret_cast<void **>(&state.sel_dev), state.sel_capacity * sizeof(uint32_t)) == cudaSuccess;
-			};
-			if (!ensure_sel(n)) {
-				b200_batch_free(batch);
-				throw OutOfMemoryException("b200: cannot allocate the probe selection buffer");
-			}
+			state.ReserveSel(n, batch);
 			rc = b200_join_probe(g.join, batch, key_cols.data(), key_cols.data(), 0, n, &out, state.sel_dev, &count);
 			if (rc == B200_ERR_CAPACITY) {
 				rc = b200_join_probe(g.join, batch, key_cols.data(), key_cols.data(), 0, 0, &out, nullptr, &count);
 				if (rc == B200_OK) {
 					b200_batch_free(out);
 					out = nullptr;
-					if (!ensure_sel(count)) {
-						b200_batch_free(batch);
-						throw OutOfMemoryException("b200: cannot allocate the probe selection buffer");
-					}
+					state.ReserveSel(count, batch);
 					rc = b200_join_probe(g.join, batch, key_cols.data(), key_cols.data(), 0, count, &out, state.sel_dev, &count);
 				}
 			}
@@ -528,11 +450,6 @@ public:
 	bool EmitNextMark(B200JoinOperatorState &state, DataChunk &chunk) const {
 		B200Timer timer(B200_T_EMIT);
 		if (state.emit_chunk >= state.buffered.size()) {
-			state.buffered.clear();
-			state.chunk_start.clear();
-			state.buffered_rows = 0;
-			state.draining = false;
-			chunk.SetCardinality(0);
 			return false;
 		}
 		idx_t c = state.emit_chunk++;
@@ -562,7 +479,7 @@ public:
 		return true;
 	}
 
-	//! emit the next <= 2048 result rows; returns false when the batch is drained (buffers are released)
+	//! emit the next <= 2048 result rows; returns false when the batch is drained
 	bool EmitNext(B200JoinOperatorState &state, DataChunk &chunk) const {
 		if (plan.join_type == B200_JOIN_MARK) {
 			return EmitNextMark(state, chunk);
@@ -574,11 +491,6 @@ public:
 			state.emit_pos = 0;
 		}
 		if (state.emit_chunk >= state.buffered.size()) {
-			state.buffered.clear();
-			state.chunk_start.clear();
-			state.buffered_rows = 0;
-			state.draining = false;
-			chunk.SetCardinality(0);
 			return false;
 		}
 		idx_t c = state.emit_chunk;
@@ -642,18 +554,9 @@ public:
 			return inner.Execute(context, input, chunk, gstate, *state.inner);
 		}
 		auto &g = sink_state->Cast<B200JoinGlobalState>();
-		if (!state.input_taken) {
-			BufferInput(context, state, input);
-			state.input_taken = true;
-			if (state.buffered_rows >= B200_PROBE_BATCH) {
-				ProbeBatch(context, g, state);
-			}
-		}
-		if (state.draining && EmitNext(state, chunk)) {
-			return OperatorResultType::HAVE_MORE_OUTPUT; // called again with the same input (already buffered)
-		}
-		state.input_taken = false;
-		return OperatorResultType::NEED_MORE_INPUT;
+		return state.Execute(
+		    context, input, chunk, B200_PROBE_BATCH, [&](b200_batch *batch) { ProbeBatch(g, state, batch); },
+		    [&](DataChunk &out) { return EmitNext(state, out); });
 	}
 
 	OperatorFinalizeResultType FinalExecute(ExecutionContext &context, DataChunk &chunk, GlobalOperatorState &gstate,
@@ -663,13 +566,9 @@ public:
 			return inner.FinalExecute(context, chunk, gstate, *state.inner);
 		}
 		auto &g = sink_state->Cast<B200JoinGlobalState>();
-		if (!state.draining && state.buffered_rows > 0) {
-			ProbeBatch(context, g, state);
-		}
-		if (state.draining && EmitNext(state, chunk)) {
-			return OperatorFinalizeResultType::HAVE_MORE_OUTPUT;
-		}
-		return OperatorFinalizeResultType::FINISHED;
+		return state.FinalExecute(
+		    context, chunk, [&](b200_batch *batch) { ProbeBatch(g, state, batch); },
+		    [&](DataChunk &out) { return EmitNext(state, out); });
 	}
 
 	// ------------------------------------------------------------------ source (host mode: external hash join)
@@ -681,16 +580,16 @@ public:
 	}
 
 	unique_ptr<GlobalSourceState> GetGlobalSourceState(ClientContext &context) const override {
-		auto state = make_uniq<B200JoinSourceState>();
+		auto state = make_uniq<B200SourceState>();
 		if (!on_device) {
 			state->inner = inner.GetGlobalSourceState(context);
 		}
 		return std::move(state);
 	}
 	unique_ptr<LocalSourceState> GetLocalSourceState(ExecutionContext &context, GlobalSourceState &gstate) const override {
-		auto state = make_uniq<B200JoinLocalSourceState>();
+		auto state = make_uniq<B200LocalSourceState>();
 		if (!on_device) {
-			state->inner = inner.GetLocalSourceState(context, *gstate.Cast<B200JoinSourceState>().inner);
+			state->inner = inner.GetLocalSourceState(context, *gstate.Cast<B200SourceState>().inner);
 		}
 		return std::move(state);
 	}
@@ -699,8 +598,8 @@ public:
 		if (on_device) {
 			return SourceResultType::FINISHED;
 		}
-		OperatorSourceInput inner_input {*input.global_state.Cast<B200JoinSourceState>().inner,
-		                                 *input.local_state.Cast<B200JoinLocalSourceState>().inner, input.interrupt_state};
+		OperatorSourceInput inner_input {*input.global_state.Cast<B200SourceState>().inner,
+		                                 *input.local_state.Cast<B200LocalSourceState>().inner, input.interrupt_state};
 		return inner.GetData(context, chunk, inner_input);
 	}
 };

@@ -16,7 +16,7 @@ threads=1, so one worker sees every chunk in table order and the batch arithmeti
     input chunk; the build side is flushed to the device every B200_MORSEL_ROWS = 1 048 576 rows;
   - hash aggregate: morsels of 1 048 576 rows cycle through a ring of two pinned buffers, Combine sinks the last two;
     the result is converted chunk by chunk (HUGEINT / BIGINT sums, integer AVG with the DECIMAL scale, NULLs);
-  - filter: batches of B200_FILTER_BATCH rows (0 = the per-chunk operator).
+  - filter: batches of B200_FILTER_BATCH rows (below one chunk, 0 included, one chunk per kernel call).
 A second pass at threads=4 covers the pooled contexts, the per-worker rings and the parallel Combine.
 
 Without a CUDA device every decorator forwards to the stock operator: the plumbing tests run the same queries, check
@@ -31,7 +31,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 EXT = os.path.join(ROOT, "integration", "_build", "libb200_duckdb.so")
 
 PROBE_BATCH = 128 * 1024      # B200_PROBE_BATCH, integration/b200_join.cpp
-MORSEL_ROWS = 1 << 20         # B200_MORSEL_ROWS, integration/b200_aggregate.cpp
+MORSEL_ROWS = 1 << 20         # B200_MORSEL_ROWS, integration/b200_binding.hpp
 PROBE_SIZES = [PROBE_BATCH - 1, PROBE_BATCH, PROBE_BATCH + 1, 2 * PROBE_BATCH + 5, 1000003]
 AGG_ROWS = 5000000
 FILTER_ROWS = 1000003
