@@ -106,6 +106,8 @@ def lib():
     L.b200_filter_project.argtypes = [vp, vp, C.POINTER(ExprNode), C.c_int, C.c_int, intp, C.c_int, C.POINTER(vp),
                                       vp, vp, u64p]
     L.b200_agg_create.argtypes = [vp, i32p, C.c_int, C.POINTER(AggDesc), C.c_int, C.c_uint64, C.POINTER(vp)]
+    L.b200_agg_create_filtered.argtypes = [vp, i32p, C.c_int, C.POINTER(AggDesc), i32p, C.c_int, C.c_uint64,
+                                           C.POINTER(vp)]
     L.b200_agg_sink.argtypes = [vp, vp, intp, intp]
     L.b200_agg_group_count.argtypes = [vp, u64p]
     L.b200_agg_export_states.argtypes = [vp, C.POINTER(vp)]
@@ -138,7 +140,7 @@ EXPORTED_SYMBOLS = [
     "b200_last_error", "b200_version", "b200_device_count", "b200_ctx_create", "b200_ctx_destroy", "b200_ctx_sync",
     "b200_ctx_stats", "b200_host_alloc", "b200_host_free", "b200_host_trim", "b200_batch_upload", "b200_batch_upload_to", "b200_batch_wrap", "b200_batch_rows",
     "b200_batch_cols", "b200_batch_column", "b200_batch_download", "b200_batch_free", "b200_hash",
-    "b200_filter_project", "b200_agg_create", "b200_agg_sink", "b200_agg_group_count", "b200_agg_export_states",
+    "b200_filter_project", "b200_agg_create", "b200_agg_create_filtered", "b200_agg_sink", "b200_agg_group_count", "b200_agg_export_states",
     "b200_agg_combine_states", "b200_agg_packed_words", "b200_agg_export_packed", "b200_agg_combine_packed",
     "b200_agg_finalize", "b200_agg_destroy", "b200_join_create", "b200_join_build_sink",
     "b200_join_finalize", "b200_join_build_rows", "b200_join_probe", "b200_join_probe_mark", "b200_join_destroy", "b200_radix_partition",

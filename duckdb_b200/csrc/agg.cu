@@ -78,7 +78,21 @@ struct b200_agg {
 	// combine_packed, fix_cnt, growth, the merge of the high-cardinality table)
 	uint64_t last_groups;
 	bool counts_fresh;
+	// the columns of b200_agg_sink's input_cols list behind each internal input (b200_agg_create_filtered): internal
+	// input i reads column in_col[i] and, when filter_col[i] >= 0, only the rows where B200_BOOL column filter_col[i]
+	// is valid and nonzero.  Without filters in_col[i] == i and filter_col[i] == -1.
+	int ncols; // entries of input_cols
+	int in_col[MAX_INPUTS];
+	int filter_col[MAX_INPUTS];
+	int nfiltered; // internal inputs with a filter
 };
+
+// columns an input_cols list of b200_agg_create_filtered may name: every distinct (input, filter) pair reads at most two
+#define MAX_AGG_COLS (2 * MAX_INPUTS)
+
+// agg_filter.cu: the validity fold of the filtered inputs (one launch per sink call)
+int b200_agg_filter_fold(b200_ctx *ctx, const DCol *in, const DCol *filt, int npairs, uint64_t n, DCol *out,
+                         void **scratch);
 
 // packed key word 0 of every group (PRIV's direct addressing tables are built from them)
 __global__ void agg_list_keys_kernel(const uint64_t *slots, uint64_t capacity, int stride, uint64_t *out, unsigned int max_out,
@@ -517,23 +531,17 @@ static int agg_grow(b200_agg *agg, uint64_t min_capacity) {
 	return B200_OK;
 }
 
-extern "C" {
-
-int b200_agg_create(b200_ctx *ctx, const int32_t *key_types, int nkeys, const b200_agg_desc *aggs, int naggs,
-                    uint64_t expected_groups, b200_agg **out) {
-	if (!ctx || !out || nkeys < 1 || nkeys > MAX_KEYS || !key_types || naggs < 0 || naggs > MAX_AGGS ||
-	    (naggs > 0 && !aggs)) {
-		b200_set_error("b200_agg_create: bad arguments (1..%d keys, 0..%d aggregates)", MAX_KEYS, MAX_AGGS);
-		return B200_ERR_INVALID;
-	}
-	AggLayout L;
+// Validate the key types and the aggregate list and lay out the slot row.  Host only: touches neither a context nor
+// CUDA, so every argument error is reported without a device.
+static int agg_layout(const char *who, const int32_t *key_types, int nkeys, const b200_agg_desc *aggs, int naggs,
+                      AggLayout &L) {
 	memset(&L, 0, sizeof(L));
 	L.nkeys = nkeys;
 	int off = 0;
 	for (int j = 0; j < nkeys; j++) {
 		int sz = b200_type_size(key_types[j]);
 		if (!sz || key_types[j] == B200_INT128) {
-			b200_set_error("b200_agg_create: unsupported key type %d", key_types[j]);
+			b200_set_error("%s: unsupported key type %d", who, key_types[j]);
 			return B200_ERR_INVALID;
 		}
 		if ((off & 7) + sz > 8) {
@@ -548,7 +556,7 @@ int b200_agg_create(b200_ctx *ctx, const int32_t *key_types, int nkeys, const b2
 	L.key_bytes = off;
 	L.key_words = (off + 7) / 8;
 	if (L.key_words > KEY_WORDS_MAX) {
-		b200_set_error("b200_agg_create: packed group key of %d bytes exceeds %d", off, KEY_WORDS_MAX * 8);
+		b200_set_error("%s: packed group key of %d bytes exceeds %d", who, off, KEY_WORDS_MAX * 8);
 		return B200_ERR_INVALID;
 	}
 	L.naggs = naggs;
@@ -557,7 +565,7 @@ int b200_agg_create(b200_ctx *ctx, const int32_t *key_types, int nkeys, const b2
 	for (int a = 0; a < naggs; a++) {
 		int f = aggs[a].func, t = aggs[a].input_type, in = aggs[a].input;
 		if (f < B200_AGG_COUNT_STAR || f > B200_AGG_AVG) {
-			b200_set_error("b200_agg_create: unknown aggregate function %d", f);
+			b200_set_error("%s: unknown aggregate function %d", who, f);
 			return B200_ERR_INVALID;
 		}
 		L.func[a] = f;
@@ -567,19 +575,19 @@ int b200_agg_create(b200_ctx *ctx, const int32_t *key_types, int nkeys, const b2
 			continue;
 		}
 		if (!b200_type_size(t) || t == B200_INT128) {
-			b200_set_error("b200_agg_create: unsupported aggregate input type %d", t);
+			b200_set_error("%s: unsupported aggregate input type %d", who, t);
 			return B200_ERR_INVALID;
 		}
 		if (f == B200_AGG_SUM_NO_OVERFLOW && !b200_type_is_integer(t)) {
-			b200_set_error("b200_agg_create: sum_no_overflow needs an integer input");
+			b200_set_error("%s: sum_no_overflow needs an integer input", who);
 			return B200_ERR_INVALID;
 		}
 		if (in < 0 || in >= MAX_INPUTS) {
-			b200_set_error("b200_agg_create: aggregate %d: input index %d out of range [0,%d)", a, in, MAX_INPUTS);
+			b200_set_error("%s: aggregate %d: input index %d out of range [0,%d)", who, a, in, MAX_INPUTS);
 			return B200_ERR_INVALID;
 		}
 		if (L.input_type[in] && L.input_type[in] != t) {
-			b200_set_error("b200_agg_create: aggregates sharing input %d disagree on its type (%d vs %d)", in,
+			b200_set_error("%s: aggregates sharing input %d disagree on its type (%d vs %d)", who, in,
 			               L.input_type[in], t);
 			return B200_ERR_INVALID;
 		}
@@ -595,7 +603,7 @@ int b200_agg_create(b200_ctx *ctx, const int32_t *key_types, int nkeys, const b2
 	}
 	for (int i = 0; i < L.ninputs; i++) {
 		if (!L.input_type[i]) {
-			b200_set_error("b200_agg_create: input %d is not used by any aggregate (inputs must be dense)", i);
+			b200_set_error("%s: input %d is not used by any aggregate (inputs must be dense)", who, i);
 			return B200_ERR_INVALID;
 		}
 	}
@@ -617,10 +625,20 @@ int b200_agg_create(b200_ctx *ctx, const int32_t *key_types, int nkeys, const b2
 	}
 	L.hash_off = w++; // the full 64-bit hash (used when the table grows)
 	L.stride = (w + 3) & ~3;
+	return B200_OK;
+}
+
+// the aggregate's table and counters on the context's device, for a layout agg_layout accepted
+static int agg_new(b200_ctx *ctx, const AggLayout &L, uint64_t expected_groups, b200_agg **out) {
 	b200_agg *agg = new b200_agg();
 	memset((void *)agg, 0, sizeof(*agg));
 	agg->ctx = ctx;
 	agg->L = L;
+	agg->ncols = L.ninputs;
+	for (int i = 0; i < L.ninputs; i++) {
+		agg->in_col[i] = i;
+		agg->filter_col[i] = -1;
+	}
 	cudaSetDevice(ctx->device);
 	uint64_t cap = next_pow2(expected_groups ? expected_groups * 2 + 16 : 1 << 16);
 	if (cap < (1 << 16)) {
@@ -650,6 +668,132 @@ int b200_agg_create(b200_ctx *ctx, const int32_t *key_types, int nkeys, const b2
 	agg->path_groups = (int)(expected_groups < 1024 ? expected_groups : 1024);
 	agg->path_groups_hc = expected_groups;
 	agg->path_decided = false;
+	*out = agg;
+	return B200_OK;
+}
+
+// an aggregate handle only exists where a context could be created: without a device the arguments are checked and the
+// call fails before the context is read
+static int agg_require_device(const char *who) {
+	if (b200_device_count() <= 0) {
+		b200_set_error("%s: no CUDA device available (there is no CPU fallback)", who);
+		return B200_ERR_NO_DEVICE;
+	}
+	return B200_OK;
+}
+
+extern "C" {
+
+int b200_agg_create(b200_ctx *ctx, const int32_t *key_types, int nkeys, const b200_agg_desc *aggs, int naggs,
+                    uint64_t expected_groups, b200_agg **out) {
+	if (!ctx || !out || nkeys < 1 || nkeys > MAX_KEYS || !key_types || naggs < 0 || naggs > MAX_AGGS ||
+	    (naggs > 0 && !aggs)) {
+		b200_set_error("b200_agg_create: bad arguments (1..%d keys, 0..%d aggregates)", MAX_KEYS, MAX_AGGS);
+		return B200_ERR_INVALID;
+	}
+	AggLayout L;
+	B200_TRY(agg_layout("b200_agg_create", key_types, nkeys, aggs, naggs, L));
+	return agg_new(ctx, L, expected_groups, out);
+}
+
+int b200_agg_create_filtered(b200_ctx *ctx, const int32_t *key_types, int nkeys, const b200_agg_desc *aggs,
+                              const int32_t *filters, int naggs, uint64_t expected_groups, b200_agg **out) {
+	const char *who = "b200_agg_create_filtered";
+	if (!ctx || !out || nkeys < 1 || nkeys > MAX_KEYS || !key_types || naggs < 0 || naggs > MAX_AGGS ||
+	    (naggs > 0 && !aggs)) {
+		b200_set_error("%s: bad arguments (1..%d keys, 0..%d aggregates)", who, MAX_KEYS, MAX_AGGS);
+		return B200_ERR_INVALID;
+	}
+	bool any_filter = false;
+	for (int a = 0; filters && a < naggs; a++) {
+		if (filters[a] < -1 || filters[a] >= MAX_AGG_COLS) {
+			b200_set_error("%s: aggregate %d: filter column %d out of range [-1,%d)", who, a, filters[a], MAX_AGG_COLS);
+			return B200_ERR_INVALID;
+		}
+		any_filter = any_filter || filters[a] >= 0;
+	}
+	AggLayout L;
+	if (!any_filter) {
+		// exactly the aggregate b200_agg_create makes
+		B200_TRY(agg_layout(who, key_types, nkeys, aggs, naggs, L));
+		B200_TRY(agg_require_device(who));
+		return agg_new(ctx, L, expected_groups, out);
+	}
+	// one internal input per distinct (input column, filter column) pair, in order of first appearance; COUNT_STAR
+	// with filter f is COUNT over the pair (f, f)
+	b200_agg_desc internal[MAX_AGGS];
+	int pair_in[MAX_INPUTS], pair_filter[MAX_INPUTS], npairs = 0;
+	int col_type[MAX_AGG_COLS] = {0};
+	for (int a = 0; a < naggs; a++) {
+		internal[a] = aggs[a];
+		int f = aggs[a].func, in = aggs[a].input, flt = filters[a];
+		if (f < B200_AGG_COUNT_STAR || f > B200_AGG_AVG) {
+			b200_set_error("%s: unknown aggregate function %d", who, f);
+			return B200_ERR_INVALID;
+		}
+		if (f == B200_AGG_COUNT_STAR) {
+			if (flt < 0) {
+				continue;
+			}
+			internal[a].func = B200_AGG_COUNT;
+			internal[a].input_type = B200_BOOL;
+			in = flt;
+		} else if (in < 0 || in >= MAX_AGG_COLS) {
+			b200_set_error("%s: aggregate %d: input index %d out of range [0,%d)", who, a, in, MAX_AGG_COLS);
+			return B200_ERR_INVALID;
+		}
+		int t = internal[a].input_type;
+		if (col_type[in] && col_type[in] != t) {
+			b200_set_error("%s: column %d is read as type %d and as type %d (a filter column is B200_BOOL)", who, in,
+			               col_type[in], t);
+			return B200_ERR_INVALID;
+		}
+		col_type[in] = t;
+		if (flt >= 0) {
+			if (col_type[flt] && col_type[flt] != B200_BOOL) {
+				b200_set_error("%s: column %d is a filter and must be B200_BOOL, an aggregate reads it as type %d", who,
+				               flt, col_type[flt]);
+				return B200_ERR_INVALID;
+			}
+			col_type[flt] = B200_BOOL;
+		}
+		int p = 0;
+		while (p < npairs && (pair_in[p] != in || pair_filter[p] != flt)) {
+			p++;
+		}
+		if (p == npairs) {
+			if (npairs == MAX_INPUTS) {
+				b200_set_error("%s: more than %d distinct (input, filter) pairs", who, MAX_INPUTS);
+				return B200_ERR_INVALID;
+			}
+			pair_in[npairs] = in;
+			pair_filter[npairs++] = flt;
+		}
+		internal[a].input = p;
+	}
+	int ncols = 0;
+	for (int c = 0; c < MAX_AGG_COLS; c++) {
+		if (col_type[c]) {
+			ncols = c + 1;
+		}
+	}
+	for (int c = 0; c < ncols; c++) {
+		if (!col_type[c]) {
+			b200_set_error("%s: column %d is neither an input nor a filter of any aggregate (the input_cols list must be "
+			               "dense)", who, c);
+			return B200_ERR_INVALID;
+		}
+	}
+	B200_TRY(agg_layout(who, key_types, nkeys, internal, naggs, L));
+	B200_TRY(agg_require_device(who));
+	b200_agg *agg = nullptr;
+	B200_TRY(agg_new(ctx, L, expected_groups, &agg));
+	agg->ncols = ncols;
+	for (int i = 0; i < npairs; i++) {
+		agg->in_col[i] = pair_in[i];
+		agg->filter_col[i] = pair_filter[i];
+		agg->nfiltered += pair_filter[i] >= 0 ? 1 : 0;
+	}
 	*out = agg;
 	return B200_OK;
 }
@@ -881,47 +1025,10 @@ static void avg_finish(int in_type, const uint64_t *raw, double *res, uint64_t g
 	}
 }
 
-extern "C" {
-
-int b200_agg_sink(b200_agg *agg, const b200_batch *in, const int *key_cols, const int *input_cols) {
-	if (!agg || !in || !key_cols || (agg->L.ninputs > 0 && !input_cols)) {
-		b200_set_error("b200_agg_sink: bad arguments");
-		return B200_ERR_INVALID;
-	}
+// b200_agg_sink behind its column set-up: n >= 1 rows of the key columns and one column per internal input
+static int agg_sink_cols(b200_agg *agg, const KeyCols &keys, AggCols &ac, uint64_t n) {
 	b200_ctx *ctx = agg->ctx;
 	const AggLayout &L = agg->L;
-	KeyCols keys;
-	B200_TRY(b200_fill_keycols(in, key_cols, L.nkeys, &keys, "b200_agg_sink"));
-	for (int j = 0; j < L.nkeys; j++) {
-		if (keys.c[j].type != L.key_type[j]) {
-			b200_set_error("b200_agg_sink: key %d has type %d, aggregate was created with %d", j, keys.c[j].type,
-			               L.key_type[j]);
-			return B200_ERR_INVALID;
-		}
-	}
-	AggCols ac;
-	memset(&ac, 0, sizeof(ac));
-	for (int i = 0; i < L.ninputs; i++) {
-		if (input_cols[i] < 0 || input_cols[i] >= (int)in->cols.size()) {
-			b200_set_error("b200_agg_sink: aggregate input %d: column %d out of range", i, input_cols[i]);
-			return B200_ERR_INVALID;
-		}
-		ac.c[i] = in->cols[input_cols[i]];
-		if (ac.c[i].type != L.input_type[i]) {
-			b200_set_error("b200_agg_sink: aggregate input %d has type %d, expected %d", i, ac.c[i].type,
-			               L.input_type[i]);
-			return B200_ERR_INVALID;
-		}
-	}
-	uint64_t n = in->nrows;
-	if (n == 0) {
-		return B200_OK;
-	}
-	if (n > 0xffffffffULL) {
-		b200_set_error("b200_agg_sink: at most 2^32-1 rows per batch");
-		return B200_ERR_INVALID;
-	}
-	CUDA_TRY(cudaSetDevice(ctx->device));
 	agg->counts_fresh = false;
 	// inputs that arrive with a validity mask for the first time: start tracking cnt(x)
 	for (int i = 0; i < L.ninputs; i++) {
@@ -1077,6 +1184,82 @@ int b200_agg_sink(b200_agg *agg, const b200_batch *in, const int *key_cols, cons
 		begin = end;
 	}
 	return B200_OK;
+}
+
+extern "C" {
+
+int b200_agg_sink(b200_agg *agg, const b200_batch *in, const int *key_cols, const int *input_cols) {
+	if (!agg || !in || !key_cols || (agg->ncols > 0 && !input_cols)) {
+		b200_set_error("b200_agg_sink: bad arguments");
+		return B200_ERR_INVALID;
+	}
+	b200_ctx *ctx = agg->ctx;
+	const AggLayout &L = agg->L;
+	KeyCols keys;
+	B200_TRY(b200_fill_keycols(in, key_cols, L.nkeys, &keys, "b200_agg_sink"));
+	for (int j = 0; j < L.nkeys; j++) {
+		if (keys.c[j].type != L.key_type[j]) {
+			b200_set_error("b200_agg_sink: key %d has type %d, aggregate was created with %d", j, keys.c[j].type,
+			               L.key_type[j]);
+			return B200_ERR_INVALID;
+		}
+	}
+	for (int c = 0; c < agg->ncols; c++) {
+		if (input_cols[c] < 0 || input_cols[c] >= (int)in->cols.size()) {
+			b200_set_error("b200_agg_sink: aggregate input %d: column %d out of range", c, input_cols[c]);
+			return B200_ERR_INVALID;
+		}
+	}
+	AggCols ac;
+	memset(&ac, 0, sizeof(ac));
+	DCol fold_in[MAX_INPUTS], fold_filter[MAX_INPUTS];
+	for (int i = 0; i < L.ninputs; i++) {
+		ac.c[i] = in->cols[input_cols[agg->in_col[i]]];
+		if (ac.c[i].type != L.input_type[i]) {
+			b200_set_error("b200_agg_sink: aggregate input %d has type %d, expected %d", agg->in_col[i], ac.c[i].type,
+			               L.input_type[i]);
+			return B200_ERR_INVALID;
+		}
+		if (agg->filter_col[i] >= 0) {
+			const DCol &f = in->cols[input_cols[agg->filter_col[i]]];
+			if (f.type != B200_BOOL) {
+				b200_set_error("b200_agg_sink: filter column %d has type %d, expected B200_BOOL", agg->filter_col[i],
+				               f.type);
+				return B200_ERR_INVALID;
+			}
+		}
+	}
+	uint64_t n = in->nrows;
+	if (n == 0) {
+		return B200_OK;
+	}
+	if (n > 0xffffffffULL) {
+		b200_set_error("b200_agg_sink: at most 2^32-1 rows per batch");
+		return B200_ERR_INVALID;
+	}
+	CUDA_TRY(cudaSetDevice(ctx->device));
+	if (agg->nfiltered == 0) {
+		return agg_sink_cols(agg, keys, ac, n);
+	}
+	// FILTER (WHERE ...): one fold gives every filtered input the validity "input valid and filter TRUE"; its scratch
+	// block is freed stream-ordered behind the sink's kernels
+	int nf = 0, fold_at[MAX_INPUTS];
+	for (int i = 0; i < L.ninputs; i++) {
+		if (agg->filter_col[i] >= 0) {
+			fold_in[nf] = ac.c[i];
+			fold_filter[nf] = in->cols[input_cols[agg->filter_col[i]]];
+			fold_at[nf++] = i;
+		}
+	}
+	DCol folded[MAX_INPUTS];
+	void *scratch = nullptr;
+	B200_TRY(b200_agg_filter_fold(ctx, fold_in, fold_filter, nf, n, folded, &scratch));
+	for (int k = 0; k < nf; k++) {
+		ac.c[fold_at[k]] = folded[k];
+	}
+	int rc = agg_sink_cols(agg, keys, ac, n);
+	b200_dev_free(ctx, scratch);
+	return rc;
 }
 
 int b200_agg_group_count(b200_agg *agg, uint64_t *out_groups) {

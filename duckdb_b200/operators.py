@@ -301,10 +301,12 @@ class HashAggregate:
     Mirrors PhysicalHashAggregate::{Sink,Combine,Finalize,GetDataInternal}
     (physical_hash_aggregate.cpp:415,503,838,958)."""
 
-    def __init__(self, ctx, key_types, aggs, expected_groups=0):
+    def __init__(self, ctx, key_types, aggs, expected_groups=0, filters=None):
         """aggs: list of (func, input_type, input) - `input` is the index of the aggregate's argument in the
         input_cols list passed to sink() (aggregates over the same column share it); -1 for COUNT_STAR.
-        2-tuples (func, input_type) get one input each, in order."""
+        2-tuples (func, input_type) get one input each, in order.
+        filters: None (b200_agg_create), or one entry per aggregate: -1, or the index in input_cols of a BOOL column -
+        the aggregate sees only the rows where it is valid and nonzero (FILTER (WHERE ...), b200_agg_create_filtered)."""
         self.ctx = ctx
         self.key_types = list(key_types)
         full, nxt = [], 0
@@ -317,13 +319,21 @@ class HashAggregate:
                 full.append((a[0], a[1], nxt))
                 nxt += 1
         self.aggs = full
-        self.ninputs = 1 + max([a[2] for a in full] + [-1])
+        self.filters = None if filters is None else [int(f) for f in filters]
+        self.ninputs = 1 + max([a[2] for a in full] + (self.filters or []) + [-1])
         descs = (capi.AggDesc * max(1, len(full)))()
         for i, (f, t, inp) in enumerate(full):
             descs[i].func, descs[i].input_type, descs[i].input, descs[i].reserved = f, t, inp, 0
         self.handle = C.c_void_p()
-        check(lib().b200_agg_create(ctx.handle, capi.i32_array(self.key_types), len(self.key_types), descs, len(aggs),
-                                    expected_groups, C.byref(self.handle)))
+        if self.filters is None:
+            check(lib().b200_agg_create(ctx.handle, capi.i32_array(self.key_types), len(self.key_types), descs,
+                                        len(aggs), expected_groups, C.byref(self.handle)))
+        else:
+            if len(self.filters) != len(full):
+                raise B200Error(capi.ERR_INVALID, "HashAggregate: one filter entry per aggregate")
+            check(lib().b200_agg_create_filtered(ctx.handle, capi.i32_array(self.key_types), len(self.key_types), descs,
+                                                 capi.i32_array(self.filters), len(aggs), expected_groups,
+                                                 C.byref(self.handle)))
 
     def sink(self, batch, key_cols, input_cols):
         """input_cols[i] = batch column of aggregate input i."""

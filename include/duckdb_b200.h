@@ -256,6 +256,24 @@ typedef struct b200_agg b200_agg; /* = GlobalSinkState of PhysicalHashAggregate 
  * expected_groups is a hint (0 = unknown); the table grows as needed. */
 B200_API int b200_agg_create(b200_ctx *ctx, const int32_t *key_types, int nkeys, const b200_agg_desc *aggs,
                              int naggs, uint64_t expected_groups, b200_agg **out);
+/* Like b200_agg_create; filters[a] = -1 (no filter) or the index, in the input_cols list of b200_agg_sink, of a
+ * B200_BOOL column: aggregate a sees only the rows where that column is valid and nonzero (FILTER (WHERE ...),
+ * physical_hash_aggregate.cpp:361-404).  filters == NULL is b200_agg_create.
+ * Every row still creates its group: SUM / MIN / MAX / AVG over no passing rows are NULL, COUNT is 0, and
+ * COUNT_STAR with filter f counts the rows where f is valid and nonzero.
+ * Aggregates share state exactly when they have the same (input, filter) pair: sum(x) and sum(x) FILTER (p) keep
+ * two sums.  Each distinct pair is one internal input; at most 12 pairs (columns used only as filters do not count).
+ * The input_cols list has 1 + max(input, filter) entries and every index must be an input or a filter; a column
+ * read both as an input and as a filter must be B200_BOOL.  b200_agg_sink returns B200_ERR_INVALID for a filter
+ * column that is not B200_BOOL.  Each sink call folds every filtered pair into one validity mask with one kernel,
+ * on the context's stream, in a scratch block it frees stream-ordered after the sink's kernels.
+ * b200_agg_export_states / b200_agg_export_packed of an aggregate with filters produce one state block per internal
+ * input, in order of first appearance of its pair in `aggs`; without filters (filters NULL or all -1) the blocks
+ * follow the input indices, as for b200_agg_create.  b200_agg_combine_states / b200_agg_combine_packed need both
+ * aggregates created with identical descs and filters.
+ * B200_ERR_INVALID for bad arguments, B200_ERR_NO_DEVICE without a CUDA device (after the arguments are checked). */
+B200_API int b200_agg_create_filtered(b200_ctx *ctx, const int32_t *key_types, int nkeys, const b200_agg_desc *aggs,
+                                      const int32_t *filters, int naggs, uint64_t expected_groups, b200_agg **out);
 /* Sink one batch: find-or-create each row's group and update the aggregate
  * states.  key_cols[k] indexes the key columns of `in`; input_cols[i] is the
  * column of `in` holding aggregate input i (i = b200_agg_desc.input; the list

@@ -5,9 +5,12 @@
 //            (src/execution/operator/aggregate/physical_hash_aggregate.cpp:415,503,838,958)
 //
 // The stock operator is planned as usual (so groups / aggregates are already reduced to BOUND_REFs of the child
-// chunk, plan_aggregate.cpp:313+); when its shape is eligible - one grouping set, no DISTINCT / FILTER, group and
-// aggregate inputs of numeric physical types, aggregates in {count_star, count, sum, sum_no_overflow, min, max,
-// avg} - it is wrapped.  With a CUDA device the wrapper batches the 2048-row chunks into morsels, uploads them
+// chunk, plan_aggregate.cpp:313+); when its shape is eligible - one grouping set, no DISTINCT, group and aggregate
+// inputs of numeric physical types, aggregates in {count_star, count, sum, sum_no_overflow, min, max, avg}, each
+// with or without a FILTER - it is wrapped.  The planner has already moved every FILTER (WHERE ...) into the
+// projection below as a BOOLEAN column (plan_aggregate.cpp:342-348), so a filter is one more staged column, and
+// b200_agg_create_filtered applies it on the device (this is also what a small PIVOT binds to: one filtered
+// aggregate per pivot value, bind_pivot.cpp:164-205).  With a CUDA device the wrapper batches the 2048-row chunks into morsels, uploads them
 // and calls b200_agg_sink; Finalize downloads [groups..., results...] and GetData emits them in <= 2048-row
 // chunks.  Without a device ("plumbing, no GPU") every call is forwarded to the wrapped stock operator.
 // Ineligible aggregates are not wrapped at all (the plan keeps the stock operator).
@@ -19,6 +22,7 @@
 #include "duckdb/common/types/hugeint.hpp"
 #include "duckdb/common/vector/flat_vector.hpp"
 
+#include <algorithm>
 #include <cmath>
 
 namespace duckdb {
@@ -33,8 +37,10 @@ struct B200AggResult {
 struct B200AggPlan {
 	bool eligible = false;
 	vector<B200Column> groups;
-	vector<B200Column> inputs; // distinct aggregate inputs
+	vector<B200Column> inputs; // distinct chunk columns the aggregates read: inputs and BOOLEAN filter columns
 	vector<b200_agg_desc> descs;
+	vector<int32_t> filters; // per desc: -1, or the index in `inputs` of its filter column
+	bool has_filter = false;
 	vector<B200AggResult> results; // one per DuckDB aggregate
 };
 
@@ -53,15 +59,40 @@ static B200AggPlan AnalyseAggregate(const PhysicalHashAggregate &op) {
 		}
 		plan.groups.push_back({group->Cast<BoundReferenceExpression>().Index(), type, GetTypeIdSize(group->GetReturnType().InternalType())});
 	}
+	// the staged column of chunk column `col` (one per chunk column, whatever reads it)
+	auto staged = [&](idx_t col, int32_t type, idx_t width) {
+		for (idx_t i = 0; i < plan.inputs.size(); i++) {
+			if (plan.inputs[i].chunk_col == col) {
+				return NumericCast<int>(i);
+			}
+		}
+		plan.inputs.push_back({col, type, width});
+		return NumericCast<int>(plan.inputs.size() - 1);
+	};
 	for (auto &expr : data.aggregates) {
 		auto &aggr = expr->Cast<BoundAggregateExpression>();
-		if (aggr.IsDistinct() || aggr.GetFilter() || aggr.GetChildren().size() > 1) {
+		if (aggr.IsDistinct() || aggr.GetChildren().size() > 1) {
 			return plan;
+		}
+		// FILTER (WHERE ...): a BOUND_REF to the BOOLEAN column the projection below computed.  The operator's
+		// constructor renumbers that reference into its payload chunk and keeps the child chunk's column in
+		// filter_indexes (physical_hash_aggregate.cpp:168-180), which is where its Sink reads it from
+		int32_t filter = -1;
+		if (aggr.GetFilter()) {
+			auto &f = *aggr.GetFilter();
+			auto entry = op.filter_indexes.find(f);
+			if (f.GetExpressionClass() != ExpressionClass::BOUND_REF || f.GetReturnType().id() != LogicalTypeId::BOOLEAN ||
+			    entry == op.filter_indexes.end()) {
+				return plan;
+			}
+			filter = staged(entry->second, B200_BOOL, 1);
+			plan.has_filter = true;
 		}
 		auto name = aggr.Function().GetName().GetIdentifierName();
 		B200AggResult res {B200AggResult::DIRECT, NumericCast<int>(plan.descs.size()), 1.0, false};
 		if (name == "count_star") {
 			plan.descs.push_back({B200_AGG_COUNT_STAR, B200_INT64, -1, 0});
+			plan.filters.push_back(filter);
 			plan.results.push_back(res);
 			continue;
 		}
@@ -73,16 +104,10 @@ static B200AggPlan AnalyseAggregate(const PhysicalHashAggregate &op) {
 		if (!B200Type(child->GetReturnType().InternalType(), in_type)) {
 			return plan;
 		}
-		idx_t col = child->Cast<BoundReferenceExpression>().Index();
-		int input = -1;
-		for (idx_t i = 0; i < plan.inputs.size(); i++) {
-			if (plan.inputs[i].chunk_col == col) {
-				input = NumericCast<int>(i);
-			}
-		}
-		if (input < 0) {
-			input = NumericCast<int>(plan.inputs.size());
-			plan.inputs.push_back({col, in_type, GetTypeIdSize(child->GetReturnType().InternalType())});
+		int input = staged(child->Cast<BoundReferenceExpression>().Index(), in_type,
+		                   GetTypeIdSize(child->GetReturnType().InternalType()));
+		if (plan.inputs[input].type != in_type) {
+			return plan; // (a BOOLEAN filter column read as an input of another physical type cannot occur)
 		}
 		bool is_float = in_type == B200_FLOAT || in_type == B200_DOUBLE;
 		auto result_physical = expr->GetReturnType().InternalType();
@@ -129,6 +154,7 @@ static B200AggPlan AnalyseAggregate(const PhysicalHashAggregate &op) {
 		} else {
 			return plan;
 		}
+		plan.filters.resize(plan.descs.size(), filter); // (AVG_INT: its SUM and COUNT carry the same filter)
 		plan.results.push_back(res);
 	}
 	// limits of b200_agg_create (MAX_AGGS / MAX_INPUTS / packed key bytes, csrc/agg.cuh)
@@ -139,7 +165,20 @@ static B200AggPlan AnalyseAggregate(const PhysicalHashAggregate &op) {
 		}
 		key_bytes += g.width;
 	}
-	if (plan.descs.size() > 16 || plan.inputs.size() > 12 || key_bytes + 1 > 32) {
+	// distinct (input, filter) pairs: the aggregate's states (count_star with filter f is the pair (f, f)); without
+	// filters these are the distinct inputs
+	vector<std::pair<int, int>> pairs;
+	for (idx_t d = 0; d < plan.descs.size(); d++) {
+		auto &desc = plan.descs[d];
+		if (desc.func == B200_AGG_COUNT_STAR && plan.filters[d] < 0) {
+			continue;
+		}
+		std::pair<int, int> pair(desc.func == B200_AGG_COUNT_STAR ? plan.filters[d] : desc.input, plan.filters[d]);
+		if (std::find(pairs.begin(), pairs.end(), pair) == pairs.end()) {
+			pairs.push_back(pair);
+		}
+	}
+	if (plan.descs.size() > 16 || pairs.size() > 12 || key_bytes + 1 > 32) {
 		return plan;
 	}
 	plan.eligible = true;
@@ -211,8 +250,14 @@ public:
 		for (auto &g : plan.groups) {
 			key_types.push_back(g.type);
 		}
-		B200Check(b200_agg_create(state->ctx, key_types.data(), NumericCast<int>(key_types.size()), plan.descs.data(),
-		                          NumericCast<int>(plan.descs.size()), 0, &state->agg));
+		if (plan.has_filter) {
+			B200Check(b200_agg_create_filtered(state->ctx, key_types.data(), NumericCast<int>(key_types.size()),
+			                                   plan.descs.data(), plan.filters.data(), NumericCast<int>(plan.descs.size()),
+			                                   0, &state->agg));
+		} else {
+			B200Check(b200_agg_create(state->ctx, key_types.data(), NumericCast<int>(key_types.size()),
+			                          plan.descs.data(), NumericCast<int>(plan.descs.size()), 0, &state->agg));
+		}
 		return std::move(state);
 	}
 
