@@ -41,6 +41,7 @@ EXPR_ADD, EXPR_SUB, EXPR_MUL, EXPR_CAST = 1001, 1002, 1003, 1004
 
 AGG_COUNT_STAR, AGG_COUNT, AGG_SUM, AGG_SUM_NO_OVERFLOW, AGG_MIN, AGG_MAX, AGG_AVG = 0, 1, 2, 3, 4, 5, 6
 JOIN_LEFT, JOIN_INNER, JOIN_SEMI, JOIN_ANTI, JOIN_MARK = 1, 3, 5, 6, 7
+JOIN_RIGHT, JOIN_OUTER = 2, 4
 
 
 class B200Error(RuntimeError):
@@ -125,6 +126,7 @@ def lib():
     L.b200_join_build_rows.argtypes = [vp, u64p]
     L.b200_join_probe.argtypes = [vp, vp, intp, intp, C.c_int, C.c_uint64, C.POINTER(vp), vp, u64p]
     L.b200_join_probe_mark.argtypes = [vp, vp, intp, vp, vp]
+    L.b200_join_scan_unmatched.argtypes = [vp, C.c_uint64, C.c_uint64, C.POINTER(vp), vp, u64p]
     L.b200_join_destroy.argtypes = [vp]
     L.b200_join_destroy.restype = None
     L.b200_radix_partition.argtypes = [vp, vp, intp, C.c_int, C.c_int, C.POINTER(vp), u64p]
@@ -143,7 +145,7 @@ EXPORTED_SYMBOLS = [
     "b200_filter_project", "b200_agg_create", "b200_agg_create_filtered", "b200_agg_sink", "b200_agg_group_count", "b200_agg_export_states",
     "b200_agg_combine_states", "b200_agg_packed_words", "b200_agg_export_packed", "b200_agg_combine_packed",
     "b200_agg_finalize", "b200_agg_destroy", "b200_join_create", "b200_join_build_sink",
-    "b200_join_finalize", "b200_join_build_rows", "b200_join_probe", "b200_join_probe_mark", "b200_join_destroy", "b200_radix_partition",
+    "b200_join_finalize", "b200_join_build_rows", "b200_join_probe", "b200_join_probe_mark", "b200_join_scan_unmatched", "b200_join_destroy", "b200_radix_partition",
     "b200_partition_count", "b200_partition_scatter", "b200_partition_count_dev", "b200_partition_scatter_dev",
 ]
 

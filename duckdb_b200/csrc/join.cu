@@ -22,6 +22,7 @@ int b200_join_probe_tile(b200_ctx *ctx, const JoinView &J, const KeyCols &keys, 
                          uint64_t n, uint64_t out_capacity, unsigned long long *counters);
 int b200_join_probe_mark_launch(b200_ctx *ctx, const JoinView &J, const KeyCols &keys, uint64_t n, uint8_t *mark,
                                 uint64_t *validity);
+int b200_join_rows_offset_launch(b200_ctx *ctx, uint32_t *rows, uint64_t n, uint32_t base);
 
 // ------------------------------------------------------------------ build
 __global__ void __launch_bounds__(256)
@@ -277,9 +278,15 @@ __global__ void __launch_bounds__(256)
 			if (first == ROW_NONE) {
 				emit_row(J, po, opos, row, ROW_NONE, 0, true);
 			} else if (J.unique) {
+				if (J.matched) {
+					J.matched[first] = 1;
+				}
 				emit_row(J, po, opos, row, first, inl, true);
 			} else {
 				for (uint32_t r = first; r != ROW_NONE; r = chain_next(J, r, ckeys)) {
+					if (J.matched) {
+						J.matched[r] = 1;
+					}
 					emit_row(J, po, opos++, row, r, inl, true);
 				}
 			}
@@ -399,7 +406,13 @@ static JoinView join_view(const b200_join *j) {
 	J.ps = j->ps;
 	J.build_has_null = j->has_null_key;
 	J.build_empty = j->rows == 0;
+	J.matched = j->matched;
 	return J;
+}
+
+// RIGHT / OUTER joins probe as INNER / LEFT; the match flags (JoinView::matched) add their build-side half
+static int probe_join_type(int join_type) {
+	return join_type == B200_JOIN_RIGHT ? B200_JOIN_INNER : join_type == B200_JOIN_OUTER ? B200_JOIN_LEFT : join_type;
 }
 
 extern "C" {
@@ -412,7 +425,8 @@ int b200_join_create(b200_ctx *ctx, int join_type, const int32_t *key_types, int
 		return B200_ERR_INVALID;
 	}
 	if (join_type != B200_JOIN_INNER && join_type != B200_JOIN_LEFT && join_type != B200_JOIN_SEMI &&
-	    join_type != B200_JOIN_ANTI && join_type != B200_JOIN_MARK) {
+	    join_type != B200_JOIN_ANTI && join_type != B200_JOIN_MARK && join_type != B200_JOIN_RIGHT &&
+	    join_type != B200_JOIN_OUTER) {
 		b200_set_error("b200_join_create: unsupported join type %d", join_type);
 		return B200_ERR_INVALID;
 	}
@@ -471,6 +485,7 @@ void b200_join_destroy(b200_join *j) {
 	b200_dev_free(ctx, j->slots);
 	b200_dev_free(ctx, j->dense);
 	b200_dev_free(ctx, j->next);
+	b200_dev_free(ctx, j->matched);
 	b200_dev_free(ctx, j->counters);
 	delete j;
 }
@@ -550,6 +565,13 @@ int b200_join_finalize(b200_join *j) {
 	}
 	b200_ctx *ctx = j->ctx;
 	CUDA_TRY(cudaSetDevice(ctx->device));
+	// RIGHT / OUTER: one match flag per build row, 0 until a probe emits the row.  Rows with a NULL key are never
+	// inserted, so their flag stays 0 and b200_join_scan_unmatched returns them (JoinHashTable::ScanFullOuter).
+	const bool outer = j->join_type == B200_JOIN_RIGHT || j->join_type == B200_JOIN_OUTER;
+	if (outer && !j->matched) {
+		B200_TRY(b200_dev_alloc(ctx, j->rows + 16, (void **)&j->matched));
+		CUDA_TRY(cudaMemsetAsync(j->matched, 0, j->rows + 16, ctx->stream));
+	}
 	// Dense (direct-addressed) table: DuckDB's perfect hash join (perfect_hash_join_executor.cpp:70-133) for a
 	// single integer key without duplicates whose range is small.  The reference caps the range at 1 M entries
 	// (:121); here 4-byte entries live in HBM/L2, so the cap is the key density (range <= 8 x rows) and 1 GiB.
@@ -579,7 +601,8 @@ int b200_join_finalize(b200_join *j) {
 						pay_bytes = 99;
 					}
 				}
-				bool inl = j->ps.n > 0 && pay_bytes <= 3 && !pay_nullable;
+				// an inline entry keeps no build row id, and RIGHT / OUTER joins flag build rows by id
+				bool inl = j->ps.n > 0 && pay_bytes <= 3 && !pay_nullable && !outer;
 				uint32_t *dense = nullptr;
 				B200_TRY(b200_dev_alloc(ctx, range * 4 + 16, (void **)&dense));
 				CUDA_TRY(cudaMemsetAsync(dense, 0, range * 4, ctx->stream));
@@ -705,7 +728,7 @@ int b200_join_probe(b200_join *j, const b200_batch *probe, const int *key_cols, 
 	*out = nullptr;
 	*out_count = 0;
 	JoinView J = join_view(j);
-	int jt = j->join_type;
+	int jt = probe_join_type(j->join_type);
 	bool with_payload = jt == B200_JOIN_INNER || jt == B200_JOIN_LEFT;
 	ProbeOut po;
 	memset(&po, 0, sizeof(po));
@@ -771,7 +794,8 @@ int b200_join_probe(b200_join *j, const b200_batch *probe, const int *key_cols, 
 		} else if (!j->dense && (j->table_cap + 1) * sizeof(JoinSlot) <= 2 * ctx->l2_persist_max) {
 			b200_l2_pin(ctx, j->slots, (j->table_cap + 1) * sizeof(JoinSlot));
 		}
-		// TMA-staged probe when the batch is eligible (single key, flat aligned columns), else the generic kernel
+		// TMA-staged probe when the batch is eligible (single key, flat aligned columns), else the generic kernel.
+		// A pass that overflows `cap` may already have set match flags; the caller's retry emits the same pairs.
 		int trc = b200_join_probe_tile(ctx, J, keys, po, jt, n, cap, j->counters);
 		if (trc == B200_ERR_INVALID) {
 			join_probe_kernel<1><<<grid, 256, 0, ctx->stream>>>(J, keys, po, jt, n, cap, j->counters);
@@ -830,6 +854,128 @@ int b200_join_probe_mark(b200_join *j, const b200_batch *probe, const int *key_c
 	}
 	CUDA_TRY(cudaSetDevice(j->ctx->device));
 	return b200_join_probe_mark_launch(j->ctx, join_view(j), keys, n, mark_dev, mark_validity_dev);
+}
+
+int b200_join_scan_unmatched(b200_join *j, uint64_t row_begin, uint64_t row_end, b200_batch **out,
+                             uint32_t *out_build_rows, uint64_t *out_count) {
+	if (!j || !out || !out_count) {
+		b200_set_error("b200_join_scan_unmatched: bad arguments");
+		return B200_ERR_INVALID;
+	}
+	// a join handle only exists where a context could be created; the check comes before the handle is read
+	if (b200_device_count() <= 0) {
+		b200_set_error("b200_join_scan_unmatched: no CUDA device available (there is no CPU fallback)");
+		return B200_ERR_NO_DEVICE;
+	}
+	if (j->join_type != B200_JOIN_RIGHT && j->join_type != B200_JOIN_OUTER) {
+		b200_set_error("b200_join_scan_unmatched: the join was created as type %d, not B200_JOIN_RIGHT or B200_JOIN_OUTER",
+		               j->join_type);
+		return B200_ERR_INVALID;
+	}
+	if (!j->finalized) {
+		b200_set_error("b200_join_scan_unmatched: call b200_join_finalize first");
+		return B200_ERR_INVALID;
+	}
+	if (row_begin % 64 != 0 || row_begin > row_end || row_end > j->rows) {
+		b200_set_error("b200_join_scan_unmatched: bad range [%llu, %llu) of %llu build rows (row_begin must be a multiple "
+		               "of 64)", (unsigned long long)row_begin, (unsigned long long)row_end, (unsigned long long)j->rows);
+		return B200_ERR_INVALID;
+	}
+	b200_ctx *ctx = j->ctx;
+	CUDA_TRY(cudaSetDevice(ctx->device));
+	*out = nullptr;
+	*out_count = 0;
+	const uint64_t n = row_end - row_begin;
+	// The scan is the filter's stream compaction over a view of the range: column 0 = the flag bytes, then the payload
+	// columns, predicate `flag = 0`, the payload columns as projections.  row_begin is a multiple of 64, so the view's
+	// validity words are the store's words from row_begin / 64 on.  A call of b200_filter_project reads at most
+	// 12 distinct columns (filter.cu's MAX_PCOLS); wider payloads are projected in slices, each selecting the same rows
+	// in the same order.
+	constexpr int SCAN_COLS = 12;
+	const int per_call = SCAN_COLS - 1;
+	b200_vector cols[MAX_PAYLOAD + 1];
+	memset(cols, 0, sizeof(cols));
+	cols[0].type = B200_UINT8;
+	cols[0].vector_type = B200_FLAT_VECTOR;
+	cols[0].data = j->matched + row_begin;
+	for (int p = 0; p < j->ps.n; p++) {
+		cols[1 + p].type = j->ps.type[p];
+		cols[1 + p].vector_type = B200_FLAT_VECTOR;
+		cols[1 + p].data = (const uint8_t *)j->ps.data[p] + row_begin * b200_type_size(j->ps.type[p]);
+		cols[1 + p].validity = j->ps.validity[p] ? j->ps.validity[p] + row_begin / 64 : nullptr;
+	}
+	b200_batch *ob = nullptr;
+	uint64_t count = 0;
+	int p0 = 0;
+	int rc = B200_OK;
+	do {
+		int np = j->ps.n - p0 < per_call ? j->ps.n - p0 : per_call;
+		b200_vector view[SCAN_COLS];
+		view[0] = cols[0];
+		b200_expr_node nodes[2 + SCAN_COLS];
+		memset(nodes, 0, sizeof(nodes));
+		nodes[0].op = B200_EXPR_COLREF;
+		nodes[0].type = B200_UINT8;
+		nodes[0].col = 0;
+		nodes[1].op = B200_EXPR_CONST;
+		nodes[1].type = B200_UINT8;
+		nodes[1].value.u = 0;
+		nodes[2].op = B200_EXPR_EQ;
+		nodes[2].type = B200_BOOL;
+		nodes[2].left = 0;
+		nodes[2].right = 1;
+		int proj[SCAN_COLS];
+		for (int q = 0; q < np; q++) {
+			view[1 + q] = cols[1 + p0 + q];
+			nodes[3 + q].op = B200_EXPR_COLREF;
+			nodes[3 + q].type = view[1 + q].type;
+			nodes[3 + q].left = nodes[3 + q].right = -1;
+			nodes[3 + q].col = 1 + q;
+			proj[q] = 3 + q;
+		}
+		nodes[0].left = nodes[0].right = nodes[1].left = nodes[1].right = -1;
+		b200_batch *in = nullptr;
+		rc = b200_batch_wrap(ctx, view, 1 + np, n, &in);
+		if (rc != B200_OK) {
+			break;
+		}
+		b200_batch *part = nullptr;
+		uint64_t c = 0;
+		rc = b200_filter_project(ctx, in, nodes, 3 + np, 2, proj, np, np ? &part : nullptr,
+		                         p0 == 0 ? out_build_rows : nullptr, nullptr, &c);
+		b200_batch_free(in);
+		if (rc != B200_OK) {
+			break;
+		}
+		count = c;
+		if (!ob) {
+			ob = part ? part : b200_batch_new(ctx, c);
+		} else {
+			// the slice's columns and the device buffers behind them move to the first slice's batch
+			ob->cols.insert(ob->cols.end(), part->cols.begin(), part->cols.end());
+			ob->dict_sizes.insert(ob->dict_sizes.end(), part->dict_sizes.begin(), part->dict_sizes.end());
+			ob->owned.insert(ob->owned.end(), part->owned.begin(), part->owned.end());
+			part->owned.clear();
+			b200_batch_free(part);
+		}
+		p0 += np;
+	} while (p0 < j->ps.n);
+	if (rc != B200_OK) {
+		b200_batch_free(ob);
+		return rc;
+	}
+	if (out_build_rows && row_begin > 0 && count > 0) {
+		// the compaction returns row ids of the view; the caller wants build row ids
+		rc = b200_join_rows_offset_launch(ctx, out_build_rows, count, (uint32_t)row_begin);
+		rc = rc ? rc : b200_ctx_sync(ctx);
+		if (rc != B200_OK) {
+			b200_batch_free(ob);
+			return rc;
+		}
+	}
+	*out = ob;
+	*out_count = count;
+	return B200_OK;
 }
 
 } // extern "C"

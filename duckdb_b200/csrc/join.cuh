@@ -50,6 +50,7 @@ struct b200_join {
 	bool unique;        // no duplicate keys
 	bool inline_payload;
 	bool has_null_key;
+	uint8_t *matched; // RIGHT / OUTER: per build row, 1 once a probe row matched it (allocated by finalize)
 	unsigned long long *counters; // device [0]=dup count, [1]=out cursor, [2]=null keys, [3] total matches
 };
 
@@ -88,6 +89,7 @@ struct JoinView {
 	PayloadStore ps;
 	bool build_has_null;
 	bool build_empty;
+	uint8_t *matched; // RIGHT / OUTER joins: the probe sets the flag of every build row it emits; NULL otherwise
 };
 
 // first build row matching the probe key of `row`, or ROW_NONE; *inl receives the slot's inline payload

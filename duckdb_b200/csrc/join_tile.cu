@@ -389,9 +389,15 @@ __global__ void __launch_bounds__(JT_THREADS, 2) join_probe_tile_kernel(const __
 			case B200_JOIN_INNER:
 			case B200_JOIN_LEFT:
 				if (first[k] == ROW_NONE || J.unique) {
+					if (J.matched && first[k] != ROW_NONE) {
+						J.matched[first[k]] = 1;
+					}
 					emit_tile_row<FAST8>(A, stage, r, prow, opos, first[k], inl[k], true);
 				} else {
 					for (uint32_t b = first[k]; b != ROW_NONE; b = J.next[b]) {
+						if (J.matched) {
+							J.matched[b] = 1;
+						}
 						emit_tile_row<FAST8>(A, stage, r, prow, opos++, b, inl[k], true);
 					}
 				}
@@ -682,8 +688,10 @@ int b200_join_probe_tile(b200_ctx *ctx, const JoinView &J, const KeyCols &keys, 
 	per_sm = per_sm < 1 ? 1 : (per_sm > 4 ? 4 : per_sm);
 	uint64_t max_grid = (uint64_t)ctx->sm_count * per_sm;
 	uint64_t grid = ntiles < max_grid ? ntiles : max_grid;
-	// lean path: INNER join on unique keys whose payload (if any) is inline in the table entry
-	bool lean = fast8 && join_type == B200_JOIN_INNER && J.unique && (J.ps.n == 0 || J.inline_payload) && J.ps.n <= 2;
+	// lean path: INNER join on unique keys whose payload (if any) is inline in the table entry.  Neither lean kernel
+	// tracks build rows, so a RIGHT join (probed as INNER, with match flags) never takes it.
+	bool lean = fast8 && join_type == B200_JOIN_INNER && !J.matched && J.unique && (J.ps.n == 0 || J.inline_payload) &&
+	            J.ps.n <= 2;
 	for (int p = 0; p < J.ps.n && p < 2; p++) {
 		A.pay_width[p] = b200_type_size(J.ps.type[p]);
 		lean = lean && A.pay_width[p] <= 2 && !po.pay_valid[p];

@@ -435,6 +435,26 @@ class HashJoin:
         words = valid_t[:(n + 63) // 64].cpu().numpy().view(np.uint64)
         return mark_t[:n].cpu().numpy(), capi.valid_from_words(words, n)
 
+    def scan_unmatched(self, row_begin=0, row_end=None, want_rows=False):
+        """RIGHT / FULL OUTER join, after the probes (b200_join_scan_unmatched): the build rows in [row_begin, row_end)
+        that no probe matched, in build-row order.  -> (Batch of the payload columns, count), plus the build row ids
+        (uint32 ndarray) when want_rows.  row_end None = every build row; row_begin must be a multiple of 64."""
+        import torch  # device buffer for the build row ids (plumbing only)
+
+        if row_end is None:
+            row_end = self.build_rows()
+        rows_t = None
+        if want_rows:
+            rows_t = torch.empty(max(row_end - row_begin, 1), dtype=torch.int32, device=f"cuda:{self.ctx.device}")
+        out = C.c_void_p()
+        count = C.c_uint64()
+        check(lib().b200_join_scan_unmatched(self.handle, row_begin, row_end, C.byref(out),
+                                             C.c_void_p(rows_t.data_ptr()) if want_rows else None, C.byref(count)))
+        batch = Batch(self.ctx, out)
+        if not want_rows:
+            return batch, count.value
+        return batch, count.value, rows_t[:count.value].cpu().numpy().view(np.uint32)
+
     def close(self):
         if self.handle:
             lib().b200_join_destroy(self.handle)

@@ -323,7 +323,9 @@ B200_API void b200_agg_destroy(b200_agg *agg);
 /* ---------------------------------------------------------------- hash join */
 typedef enum b200_join_type { /* duckdb::JoinType values (enums/join_type.hpp:18-34) */
 	B200_JOIN_LEFT = 1,
+	B200_JOIN_RIGHT = 2,
 	B200_JOIN_INNER = 3,
+	B200_JOIN_OUTER = 4, /* FULL OUTER */
 	B200_JOIN_SEMI = 5,
 	B200_JOIN_ANTI = 6,
 	B200_JOIN_MARK = 7
@@ -357,6 +359,10 @@ B200_API int b200_join_build_rows(b200_join *join, uint64_t *out_rows);
  * SEMI / ANTI: probe rows with (without) a match, lhs columns only.
  * MARK: every probe row, one extra BOOL column (NULL when the probe key is
  *       NULL) after the lhs columns.
+ * RIGHT: like INNER; OUTER (FULL): like LEFT.  Both also flag every build row
+ *       they emit, for b200_join_scan_unmatched.  A call that returns
+ *       B200_ERR_CAPACITY may have flagged rows already; its retry emits the
+ *       same rows, so the flags end up the same.
  * out_capacity bounds the result rows (B200_ERR_CAPACITY if exceeded; pass 0
  * to let the library size it exactly with a counting pass).
  * Probe key columns have the types the join was created with; lhs columns
@@ -389,6 +395,17 @@ B200_API int b200_join_probe(b200_join *join, const b200_batch *probe, const int
  * (physical_comparison_join.cpp:116-150) for an empty build side. */
 B200_API int b200_join_probe_mark(b200_join *join, const b200_batch *probe, const int *key_cols, uint8_t *mark_dev,
                                   uint64_t *mark_validity_dev);
+/* B200_JOIN_RIGHT / B200_JOIN_OUTER, after the probes: the build rows in [row_begin, row_end) that no
+ * b200_join_probe call matched (NULL-key rows included), in build-row order.  Output batch = the build
+ * payload columns; out_build_rows (device, may be NULL) receives each result row's build row index;
+ * out_count (host).  Synchronises.  row_begin must be a multiple of 64.
+ * The caller emits these rows with NULL probe-side columns.  B200_ERR_INVALID for a NULL argument, a join of
+ * another type, one not yet finalized, or a range that is not inside [0, b200_join_build_rows) or whose
+ * row_begin is not a multiple of 64; B200_ERR_NO_DEVICE without a CUDA device.  Replaces
+ * JoinHashTable::ScanFullOuter (join_hashtable.cpp:2302-2356) behind PhysicalHashJoin::GetData
+ * (physical_hash_join.cpp) for RIGHT and FULL OUTER joins. */
+B200_API int b200_join_scan_unmatched(b200_join *join, uint64_t row_begin, uint64_t row_end,
+                                      b200_batch **out, uint32_t *out_build_rows, uint64_t *out_count);
 B200_API void b200_join_destroy(b200_join *join);
 
 /* ---------------------------------------------------------- radix partition */

@@ -4,10 +4,13 @@
 //   replaces PhysicalHashJoin::{Sink,Combine,Finalize,ExecuteInternal}
 //            (src/execution/operator/join/physical_hash_join.cpp:764,840,1893,2139)
 //
-// Eligible shapes: INNER / LEFT / SEMI / ANTI, equality conditions on BOUND_REF keys of numeric physical types,
+// Eligible shapes: INNER / LEFT / RIGHT / FULL OUTER / SEMI / ANTI, equality conditions on BOUND_REF keys of numeric physical types,
 // no residual predicate, build-side output columns of numeric physical types.  Probe-side output columns may have
 // ANY type: the kernel returns the probe row id of every result row and the operator slices the input chunk with
 // it (the same contract as ScanStructure::NextInnerJoin, join_hashtable.cpp:1737-1760).
+// RIGHT and FULL OUTER joins probe like INNER and LEFT; the library flags every build row a probe emits.  Once every
+// probe has run, the operator is also a source: workers take 1 Mi-row build ranges and emit the unflagged rows of each
+// (b200_join_scan_unmatched) with NULL probe-side columns (JoinHashTable::ScanFullOuter, join_hashtable.cpp:2302-2356).
 // MARK joins (large IN lists, IN subqueries that are not plain conjuncts) with ONE such condition, uncorrelated,
 // without build-side output columns: the result is every probe row plus a BOOL mark, in probe order
 // (b200_join_probe_mark), so each buffered input chunk is emitted whole with the mark vector appended.  Several
@@ -19,6 +22,7 @@
 // the wrapped operator.
 #include "b200_binding.hpp"
 
+#include "duckdb/common/vector/constant_vector.hpp"
 #include "duckdb/common/vector/flat_vector.hpp"
 #include "duckdb/execution/operator/join/physical_hash_join.hpp"
 #include "duckdb/parallel/meta_pipeline.hpp"
@@ -43,6 +47,8 @@ static B200JoinPlan AnalyseJoin(const PhysicalHashJoin &op) {
 	switch (op.join_type) {
 	case JoinType::INNER:
 	case JoinType::LEFT:
+	case JoinType::RIGHT:
+	case JoinType::OUTER:
 	case JoinType::SEMI:
 	case JoinType::ANTI:
 	case JoinType::MARK:
@@ -72,7 +78,8 @@ static B200JoinPlan AnalyseJoin(const PhysicalHashJoin &op) {
 		plan.probe_keys.push_back({lhs.Cast<BoundReferenceExpression>().Index(), ltype, width});
 		plan.build_keys.push_back({rhs.Cast<BoundReferenceExpression>().Index(), rtype, width});
 	}
-	bool with_payload = op.join_type == JoinType::INNER || op.join_type == JoinType::LEFT;
+	bool with_payload = op.join_type == JoinType::INNER || op.join_type == JoinType::LEFT ||
+	                    op.join_type == JoinType::RIGHT || op.join_type == JoinType::OUTER;
 	if (with_payload) {
 		// rhs_output_columns index the hash table layout [keys..., payload...] (physical_hash_join.cpp:209-232)
 		idx_t nkeys = op.conditions.size();
@@ -145,6 +152,27 @@ public:
 };
 
 static constexpr idx_t B200_PROBE_BATCH = 128 * 1024;
+//! RIGHT / FULL OUTER source phase: build rows per b200_join_scan_unmatched call (a multiple of 64)
+static constexpr idx_t B200_SCAN_RANGE = 1 << 20;
+
+//! RIGHT / FULL OUTER source phase: the next build range to scan
+class B200JoinSourceState : public B200SourceState {
+public:
+	std::atomic<idx_t> next_range {0};
+	idx_t ranges = 0;
+	idx_t MaxThreads() override {
+		return inner ? inner->MaxThreads() : MaxValue<idx_t>(ranges, 1);
+	}
+};
+
+//! RIGHT / FULL OUTER source phase: the unmatched build rows of the worker's current range, on the host
+class B200JoinLocalSourceState : public B200LocalSourceState {
+public:
+	vector<vector<data_t>> payload_data;
+	vector<vector<uint64_t>> payload_valid;
+	idx_t count = 0;
+	idx_t emitted = 0;
+};
 //! MARK join block: validity words, then mark bytes, for a batch of at most one chunk past B200_PROBE_BATCH rows
 static constexpr idx_t B200_MARK_ROWS = B200_PROBE_BATCH + STANDARD_VECTOR_SIZE;
 static constexpr idx_t B200_MARK_VALID_BYTES = (B200_MARK_ROWS + 63) / 64 * 8;
@@ -572,31 +600,115 @@ public:
 	}
 
 	// ------------------------------------------------------------------ source (host mode: external hash join)
+	// ------------------------------------------------------------------ source (device: the unmatched build rows of
+	// RIGHT / FULL OUTER joins; host mode: whatever the stock operator emits, e.g. its external hash join)
+	bool EmitsBuildSide() const {
+		return plan.join_type == B200_JOIN_RIGHT || plan.join_type == B200_JOIN_OUTER;
+	}
 	bool IsSource() const override {
-		return on_device ? false : inner.IsSource();
+		return on_device ? EmitsBuildSide() : inner.IsSource();
 	}
 	bool ParallelSource() const override {
-		return !on_device;
+		return !on_device || EmitsBuildSide();
 	}
 
 	unique_ptr<GlobalSourceState> GetGlobalSourceState(ClientContext &context) const override {
-		auto state = make_uniq<B200SourceState>();
+		auto state = make_uniq<B200JoinSourceState>();
 		if (!on_device) {
 			state->inner = inner.GetGlobalSourceState(context);
+		} else if (sink_state) {
+			uint64_t rows = 0;
+			B200Check(b200_join_build_rows(sink_state->Cast<B200JoinGlobalState>().join, &rows));
+			state->ranges = (rows + B200_SCAN_RANGE - 1) / B200_SCAN_RANGE;
 		}
 		return std::move(state);
 	}
 	unique_ptr<LocalSourceState> GetLocalSourceState(ExecutionContext &context, GlobalSourceState &gstate) const override {
-		auto state = make_uniq<B200LocalSourceState>();
+		auto state = make_uniq<B200JoinLocalSourceState>();
 		if (!on_device) {
 			state->inner = inner.GetLocalSourceState(context, *gstate.Cast<B200SourceState>().inner);
+		} else {
+			state->payload_data.resize(plan.payload.size());
+			state->payload_valid.resize(plan.payload.size());
 		}
 		return std::move(state);
 	}
+
+	//! scan the next build range of this worker into its host buffers; false when every range is taken
+	bool ScanNextRange(B200JoinGlobalState &g, B200JoinSourceState &gs, B200JoinLocalSourceState &l) const {
+		idx_t range = gs.next_range++;
+		if (range >= gs.ranges) {
+			return false;
+		}
+		b200_batch *out = nullptr;
+		uint64_t count = 0;
+		int rc;
+		{
+			auto t_lock = make_uniq<B200Timer>(B200_T_LOCK_WAIT);
+			std::lock_guard<std::mutex> guard(g.lock); // one join object (one stream), driven from one thread at a time
+			t_lock.reset();
+			B200Timer timer(B200_T_KERNEL_CALL);
+			uint64_t rows = 0;
+			rc = b200_join_build_rows(g.join, &rows);
+			uint64_t begin = range * B200_SCAN_RANGE;
+			uint64_t end = MinValue<uint64_t>(begin + B200_SCAN_RANGE, rows);
+			if (rc == B200_OK) {
+				rc = b200_join_scan_unmatched(g.join, begin, end, &out, nullptr, &count);
+			}
+			for (idx_t p = 0; p < plan.payload.size() && rc == B200_OK; p++) {
+				l.payload_data[p].resize(count * plan.payload[p].width + 16);
+				l.payload_valid[p].assign((count + 63) / 64 + 1, 0);
+				rc = b200_batch_download(g.ctx, out, NumericCast<int>(p), l.payload_data[p].data(),
+				                         l.payload_valid[p].data());
+			}
+		}
+		b200_batch_free(out);
+		B200Check(rc);
+		l.count = count;
+		l.emitted = 0;
+		return true;
+	}
+
+	//! the next <= 2048 unmatched build rows: constant NULL probe-side columns, the build columns copied as EmitNext
+	//! copies them
+	void EmitUnmatched(B200JoinLocalSourceState &l, DataChunk &chunk) const {
+		B200Timer timer(B200_T_EMIT);
+		idx_t first = l.emitted;
+		idx_t count = MinValue<idx_t>(STANDARD_VECTOR_SIZE, l.count - first);
+		idx_t nlhs = plan.lhs_output.size();
+		for (idx_t col = 0; col < nlhs; col++) {
+			chunk.data[col].SetVectorType(VectorType::CONSTANT_VECTOR);
+			ConstantVector::SetNull(chunk.data[col], true);
+		}
+		for (idx_t p = 0; p < plan.payload.size(); p++) {
+			auto &vec = chunk.data[nlhs + p];
+			idx_t width = plan.payload[p].width;
+			memcpy(FlatVector::GetDataMutable(vec), l.payload_data[p].data() + first * width, count * width);
+			auto &valid = l.payload_valid[p];
+			for (idx_t i = 0; i < count; i++) {
+				idx_t row = first + i;
+				if (!((valid[row >> 6] >> (row & 63)) & 1)) {
+					FlatVector::SetNull(vec, i, true);
+				}
+			}
+		}
+		chunk.SetCardinality(count);
+		l.emitted += count;
+	}
+
 	SourceResultType GetDataInternal(ExecutionContext &context, DataChunk &chunk,
 	                                 OperatorSourceInput &input) const override {
 		if (on_device) {
-			return SourceResultType::FINISHED;
+			auto &g = sink_state->Cast<B200JoinGlobalState>();
+			auto &gs = input.global_state.Cast<B200JoinSourceState>();
+			auto &l = input.local_state.Cast<B200JoinLocalSourceState>();
+			while (l.emitted >= l.count) {
+				if (!ScanNextRange(g, gs, l)) {
+					return SourceResultType::FINISHED;
+				}
+			}
+			EmitUnmatched(l, chunk);
+			return SourceResultType::HAVE_MORE_OUTPUT;
 		}
 		OperatorSourceInput inner_input {*input.global_state.Cast<B200SourceState>().inner,
 		                                 *input.local_state.Cast<B200LocalSourceState>().inner, input.interrupt_state};
